@@ -152,7 +152,7 @@ class HotPath:
         self.clip, self.perceiver, self.gated = build_modules(dev, cfg)
         self.trainable = list(self.perceiver.parameters()) + list(self.gated.parameters())
         mode = args.grad_comm_dtype
-        if mode == "auto":       # measured at N = 2 (profiles/r02_scale_sweep_n2.md): bf16-direct 713, fp32 688-705, bf16 664
+        if mode == "auto":       # N > 1: the bf16 wire format halves the all-reduce payload
             mode = "bf16-direct" if world > 1 else "fp32"
         self.comm_mode = mode
         comm_dtype = torch.bfloat16 if mode.startswith("bf16") else None
@@ -258,6 +258,7 @@ class HotPath:
         import torch.distributed as dist
         start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         pf = self.prefetch
+        loss = None
         if self.world > 1:
             dist.barrier()
         torch.cuda.synchronize()
@@ -280,8 +281,9 @@ class HotPath:
                 self.loss_host.copy_(loss, non_blocking=True)
                 torch.cuda.current_stream().synchronize()                   # the user reads the loss every step
             else:
-                self.run_step()
+                loss = self.run_step()
         end.record()
+        self.last_loss = loss if n > 0 else None
         if self.world > 1:
             dist.barrier()
         torch.cuda.synchronize()
@@ -304,6 +306,28 @@ class HotPath:
         import gc
         gc.collect()
         torch.cuda.empty_cache()
+
+
+def dump_outputs(hp, out_dir, n_sample=1 << 22):
+    """Write what the timed path computed in its last step as DIR/<name>.npy (float32 / float64, ~26 MB in all):
+      loss           float32 [1]      the step's loss
+      grad_sample    float32 [4 Mi]   the fp32 gradient buffer (every trainable .grad is a view of it) at fixed indices
+                                      (drawn from a CPU generator seeded with SEED, sorted)
+      grad_norms     float64 [P]      L2 norm of each trainable parameter's gradient, in parameter order
+      clip_features  float32 [bTF, 257, 1024]   the frozen CLIP tower's output the step produced
+    Inputs and weights come from fixed seeds, so two builds run with the same arguments can be compared file by file."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    flat = hp.flat.flat.view(-1)
+    g = torch.Generator().manual_seed(SEED)
+    idx = torch.randint(0, flat.numel(), (min(n_sample, flat.numel()),), generator=g).sort().values.to(flat.device)
+    arrays = {"loss": hp.last_loss.detach().float().reshape(1),
+              "grad_sample": flat[idx].float(),
+              "grad_norms": torch.stack([p.grad.detach().double().norm() for p in hp.trainable]),
+              "clip_features": hp.hidden.detach().float()}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.cpu().numpy())
 
 
 def graph_time_us(calls, reps=5):
@@ -375,7 +399,7 @@ def dominant_gemm_times(dev, M, D):
 def hbm_kernel_rooflines(dev, batch, cfg, hbm_gbs):
     """The HBM-bound kernels of the step against the measured copy bandwidth (SURVEY.md §8d): fused attention A
     (perceiver), B (gated cross-attention), their backward, the CLIP attention, LayerNorm and the weight cast.
-    Each launch of a timed graph works on its own buffers (rotating sets, > 126 MB in total) so operands come from HBM,
+    Each launch of a timed graph works on its own buffers (rotating sets, > 256 MB in total, 5x the H100's 50 MB L2) so operands come from HBM,
     not from L2; `bytes` are the ALGORITHMIC bytes (every operand touched once, SURVEY.md §8d)."""
     from otter_b200 import functional as F
     BF = torch.bfloat16
@@ -748,6 +772,9 @@ def run_cuda(args):
     log(f"timed region done: {ms / args.steps:.3f} ms/step")
     launches = hp.launches_per_step
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(hp, args.dump_outputs)
+        log(f"outputs of the last timed step written to {args.dump_outputs}")
     ms_e2e = hp.timed(args.steps, e2e=True)
 
     peaks = {}
@@ -755,7 +782,7 @@ def run_cuda(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_gbs = peaks.get("hbm_gbs", 6600.0)
+    hbm_gbs = peaks.get("hbm_gbs", 3350.0)
 
     # ---- roofline of the dominant kernel: the six 4096<->16384 FFN GEMM launch classes of the gated blocks
     # (8 launches each per step, 86 % of the step's algorithmic FLOPs), each timed live with CUDA events over
@@ -816,10 +843,10 @@ def run_cuda(args):
         if world > 1:
             dist.destroy_process_group()
         return
-    peak_tf = peaks.get("bf16_tflops", 1590.0)                # kernel timed alone -> burst figure
-    peak_sus = peaks.get("bf16_tflops_sustained", 1400.0)
+    peak_tf = peaks.get("bf16_tflops", 989.0)                 # kernel timed alone -> burst figure
+    peak_sus = peaks.get("bf16_tflops_sustained", 989.0)
     peak_src = "MEASURED_PEAKS.json bf16_tflops (burst; kernel timed alone)" if peaks else \
-        "fallback 1590 TFLOP/s (B200_PROFILING.md)"
+        "fallback 989 TFLOP/s: H100 SXM data sheet, dense BF16 at 700 W (not a measured figure)"
     step_ms = ms / args.steps
     value = batch * world * args.steps / (ms / 1e3)
     e2e_value = batch * world * args.steps / (ms_e2e / 1e3)
@@ -841,7 +868,7 @@ def run_cuda(args):
                    "weights": "fp32 master, bf16 compute copies re-cast every step; fp32 `.grad` views of one flat buffer" +
                               ("; the Linear weights' wgrad epilogues write the bf16 wire buffer of the all-reduce, one up-cast "
                                "after it" if comm_mode == "bf16-direct" else ""),
-                   "cache": "per-step working set (2.4 GB bf16 weights + activations) >> 126 MB L2; no explicit flush",
+                   "cache": "per-step working set (2.4 GB bf16 weights + activations) >> 50 MB L2; no explicit flush",
                    "grad_allreduce_bytes": comm_bytes,
                    "grad_allreduce_dtype": comm_mode, "nccl_registered_buffer": bool(args.nccl_registered),
                    "grad_allreduce_op": ("sum, 1/N folded into the up-cast" if (args.reduce_op == "sum" and comm_mode != "fp32") else "avg")},
@@ -851,14 +878,12 @@ def run_cuda(args):
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"bound": "tensor",
-                     "kernel": "otb::gemm2_bf16_kernel (tcgen05 cta_group::2 / TMA) — the six 4096<->16384 FFN GEMM classes "
+                     "kernel": "otb::gemm_bf16_kernel (wgmma / TMA) — the six 4096<->16384 FFN GEMM classes "
                                "(fwd, dgrad, wgrad) of the gated blocks, 48 launches/step",
                      "achieved": round(ach, 1), "peak": peak_tf, "unit": "TFLOP/s",
                      "frac": round(ach / peak_tf, 4) if peak_tf else None,
-                     "traffic": 259.1e6, "traffic_note": "dram read+write of one 2048x16384x4096 GELU+aux launch of "
-                                                         "gemm2_bf16_kernel (shipped epilogue), ncu --set full, "
-                                                         "profiles/r02_final_ncu_gemm_and_fused.md (algorithmic 285 MB; "
-                                                         "tensor pipe 82.7 % active)",
+                     "traffic": 285.2e6, "traffic_note": "algorithmic bytes of one 2048x16384x4096 GELU+aux launch "
+                                                         "(operands read once, output and pre-activation written once)",
                      "peak_source": peak_src, "frac_of_sustained_peak": round(ach / peak_sus, 4),
                      "per_class_us": dom["per_class_us"], "flops_per_launch_avg": dom["flops_avg"],
                      "share_of_step": round(8 * dom["sum_ms"] / step_ms, 3),
@@ -866,7 +891,7 @@ def run_cuda(args):
                      "step_algorithmic_tflops": round(fl * batch / (step_ms * 1e-3) / 1e12, 1),
                      "step_frac_of_sustained_peak": round(fl * batch / (step_ms * 1e-3) / 1e12 / peak_sus, 4),
                      "hbm_bound_kernels": {"peak_gbs": hbm_gbs, "peak_source": "MEASURED_PEAKS.json hbm_gbs" if peaks
-                                           else "fallback 6600 GB/s", "timing": "CUDA-graph replay, CUDA events, "
+                                           else "fallback 3350 GB/s (H100 SXM data sheet)", "timing": "CUDA-graph replay, CUDA events, "
                                            "rotating operand sets > L2 (cold operands)", "kernels": hbm_rows}},
     }
     if comm_alone is not None:
@@ -1075,7 +1100,12 @@ def main():
     ap.add_argument("--ref-batch", type=int, default=0, help="reference arm: batch per step (default: --per-gpu-batch)")
     ap.add_argument("--ref-budget-s", type=float, default=150.0, help="reference arm: wall-clock bound of the timed steps")
     ap.add_argument("--ref-port", action="store_true", help="reference arm: time oracle/restatement.py instead")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last one computed (loss, gradients, CLIP features) as "
+                         "DIR/<name>.npy, for comparing two builds output for output")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     BASE_CFG["L"] = args.seq_len
     if args.impl == "reference":
         run_reference(args)

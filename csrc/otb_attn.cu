@@ -1,4 +1,4 @@
-// otter_b200 — fused attention cores on tcgen05 / TMA (forward + backward).
+// otter_b200 — fused attention cores on wgmma / TMA (forward + backward).
 //
 // One kernel family serves the three attention cores of the hot path:
 //   (A) perceiver latent x (vision ++ latent) attention      modeling_otter.py:168-179   (two key sources)
@@ -8,14 +8,14 @@
 // Layout: no head permutes — Q/K/V/O are read/written in place inside the projection GEMM outputs
 // ([rows][cols] bf16, head h at columns col0 + h*64), addressed through TMA tensor maps.
 //
-// Forward, per CTA = (128-row query tile, head, problem), 128 threads (thread t owns query row t):
-//   S = Q K^T on tcgen05.mma (128x128x64) into TMEM; rows read back with tcgen05.ld; softmax in fp32
-//   registers (two sweeps over the key tiles: row max, then exp/accumulate — no rescaling of O);
-//   P (bf16) staged in 128B-swizzled smem; O += P V on tcgen05.mma with V consumed MN-major straight
-//   from its TMA tile; O/l written once.  K/V tiles are double-buffered TMA loads.
-// Backward, per CTA = (head, problem): loops key tiles (outer) x query tiles (inner) with
-//   S, dP = dO V^T, dV += P^T dO, dK += dS^T Q, dQ = dS K all on tcgen05 (P/dS staged in smem and
-//   consumed K-major and MN-major from the same bytes); dK/dV accumulate in TMEM across query tiles.
+// Forward, per CTA = (128-row query tile, head, problem), one warpgroup (thread t owns query row t):
+//   S = Q K^T on wgmma (two m64n128k16 halves) parked in a swizzled fp32 smem tile and read back row by row; softmax in
+//   fp32 registers (two sweeps over the key tiles: row max, then exp/accumulate — no rescaling of O); P (bf16) staged
+//   in 128B-swizzled smem; O += P V on wgmma with V consumed MN-major straight from its TMA tile, O accumulated in
+//   registers across key tiles; O/l written once.  K/V tiles are double-buffered TMA loads.
+// Backward, per CTA = (head, problem): loops key tiles (outer) x query tiles (inner) with S, dP = dO V^T (in two
+//   64-key halves through 32 KB fp32 tiles), dV += P^T dO, dK += dS^T Q (accumulated in registers across query tiles)
+//   and dQ = dS K, all on wgmma; P / dS are staged in smem and consumed K-major and MN-major from the same bytes.
 //
 // Mask semantics of (B) (bit-exact w.r.t. the reference, SURVEY.md §8a-5): with tt = text_time[b,row]
 //   tt == 0        -> attention row zeroed after softmax (output row exactly 0, no gradients)
@@ -42,27 +42,20 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   uint8_t* s_k = s_q + kTileBytes;            // 2 x 16 KB
   uint8_t* s_v = s_k + 2 * kTileBytes;        // 2 x 16 KB
   uint8_t* s_p = s_v + 2 * kTileBytes;        // 32 KB: P as two 64-key chunks of [128 rows][128 B]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_p + 2 * kTileBytes);
+  uint8_t* acc_s = s_p + 2 * kTileBytes;      // 64 KB: S [128][128] fp32 (O [128][64] at the end)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(acc_s + 4 * kTileBytes);
   uint64_t* full = bars;        // [2]
   uint64_t* bar_q = bars + 2;
-  uint64_t* bar_s = bars + 3;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int qt = blockIdx.x, h = blockIdx.y, prob = blockIdx.z;
 
-  if (tid == 32) {
-    mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(bar_q, 1); mbar_init(bar_s, 1);
+  if (tid == 0) {
+    mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(bar_q, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 256);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();   // predecessor grid complete before any global / TMA access
-  const uint32_t t_s = tmem;         // S: columns [0,128)
-  const uint32_t t_o = tmem + 128;   // O: columns [128,192)
 
   const int nt1 = (p.Sk1 + 127) / 128, nt2 = (p.Sk2 + 127) / 128, nt = nt1 + nt2;
   const int nsteps = (nt == 1) ? 1 : 2 * nt;
@@ -83,21 +76,26 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     tma_load_2d(s_k + st * kTileBytes, m, &full[st], (kt.src ? p.k2_col0 : p.k1_col0) + h * 64, kt.row0);
     if (need_v) tma_load_2d(s_v + st * kTileBytes, m, &full[st], (kt.src ? p.v2_col0 : p.v1_col0) + h * 64, kt.row0);
   };
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-  constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, false, true);
-  auto issue_s = [&](int st) {  // S = Q K^T
-    const uint64_t da = make_smem_desc(smem_u32(s_q), 16, 1024);
-    const uint64_t db = make_smem_desc(smem_u32(s_k + st * kTileBytes), 16, 1024);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) umma_bf16(t_s, da + k * 2, db + k * 2, idesc_s, k != 0);
+  const uint32_t q_addr = smem_u32(s_q);
+  auto compute_s = [&](int st) {  // S = Q K^T into acc_s
+    const uint32_t k_addr = smem_u32(s_k + st * kTileBytes);
+    wg_mma_tile<128, 0, 0>(
+        acc_s, 4, [&](int hh, int k) { return make_smem_desc(q_addr + hh * 8192 + k * 32, 16, 1024); },
+        [&](int k) { return make_smem_desc(k_addr + k * 32, 16, 1024); });
   };
-  auto issue_pv = [&](int st, bool accumulate) {  // O += P V   (A = P K-major over keys, B = V MN-major)
-    const uint64_t db = make_smem_desc(smem_u32(s_v + st * kTileBytes), 16, 1024);
+  float o[2][32];               // O rows [64 h, 64 h + 64) as wgmma fragments
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const uint64_t da = make_smem_desc(smem_u32(s_p + (k >> 2) * kTileBytes) + (k & 3) * 32, 16, 1024);
-      umma_bf16(t_o, da, db + k * 128, idesc_pv, (accumulate || k != 0) ? 1u : 0u);
-    }
+  for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[hh][i] = 0.f;
+  bool o_started = false;
+  auto issue_pv = [&](int st) {  // O += P V   (A = P K-major over keys, B = V MN-major)
+    const uint32_t v_addr = smem_u32(s_v + st * kTileBytes), p_addr = smem_u32(s_p);
+    wg_mma_regs<64, 0, 1>(
+        o, o_started, 8,
+        [&](int hh, int k) { return make_smem_desc(p_addr + (k >> 2) * kTileBytes + hh * 8192 + (k & 3) * 32, 16, 1024); },
+        [&](int k) { return make_smem_desc(v_addr + k * 2048, 16, 1024); });
+    o_started = true;
   };
 
   if (tid == 0) {
@@ -105,19 +103,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
     mbar_arrive_expect_tx(bar_q, kTileBytes);
     tma_load_2d(s_q, &map_q, bar_q, p.q_col0 + h * 64, prob * p.Sq + qt * 128);
     issue_load(0);
-    mbar_wait(bar_q, 0);
-    mbar_wait(&full[0], 0);
-    tc_fence_after();
-    issue_s(0);
-    umma_commit(bar_s);
   }
+  mbar_wait(bar_q, 0);
+  mbar_wait(&full[0], 0);
+  compute_s(0);
+  __syncthreads();
 
   float m_run = -INFINITY, l_run = 0.f;
-  const uint32_t lane_addr = static_cast<uint32_t>(warp * 32) << 16;
   for (int s = 0; s < nsteps; ++s) {
-    mbar_wait(bar_s, s & 1);
-    if (tid == 0 && s + 1 < nsteps) issue_load(s + 1);
-    tc_fence_after();
+    if (tid == 0 && s + 1 < nsteps) issue_load(s + 1);   // its buffer was last read by the MMAs of step s - 1
     const int j = (nt == 1) ? 0 : (s % nt);
     const bool is_p2 = (nt == 1) || (s >= nt);
     const bool do_max = (nt == 1) || (s < nt);
@@ -127,8 +121,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
         uint32_t r[32];
-        tmem_ld32(t_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32<128>(acc_s, tid, c * 32, r);
         if (cls == 1) {
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
@@ -143,8 +136,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
 #pragma unroll 1
       for (int c = 0; c < 4; ++c) {
         uint32_t r[32];
-        tmem_ld32(t_s + lane_addr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32<128>(acc_s, tid, c * 32, r);
         float pv[32];
 #pragma unroll
         for (int i = 0; i < 32; ++i) {
@@ -158,588 +150,48 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         uint8_t* chunk = s_p + (c >> 1) * kTileBytes;
 #pragma unroll
         for (int g = 0; g < 4; ++g) {
-          uint4 o;
-          o.x = pack_bf16x2(pv[g * 8 + 0], pv[g * 8 + 1]); o.y = pack_bf16x2(pv[g * 8 + 2], pv[g * 8 + 3]);
-          o.z = pack_bf16x2(pv[g * 8 + 4], pv[g * 8 + 5]); o.w = pack_bf16x2(pv[g * 8 + 6], pv[g * 8 + 7]);
-          st_sw128(chunk, tid, (c & 1) * 32 + g * 8, o);
+          uint4 ov;
+          ov.x = pack_bf16x2(pv[g * 8 + 0], pv[g * 8 + 1]); ov.y = pack_bf16x2(pv[g * 8 + 2], pv[g * 8 + 3]);
+          ov.z = pack_bf16x2(pv[g * 8 + 4], pv[g * 8 + 5]); ov.w = pack_bf16x2(pv[g * 8 + 6], pv[g * 8 + 7]);
+          st_sw128(chunk, tid, (c & 1) * 32 + g * 8, ov);
         }
       }
       fence_proxy_async_smem();
     }
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      if (is_p2) issue_pv(s & 1, (nt != 1) && (s > nt));
-      if (s + 1 < nsteps) {
-        mbar_wait(&full[(s + 1) & 1], ((s + 1) >> 1) & 1);
-        tc_fence_after();
-        issue_s((s + 1) & 1);
-      }
-      umma_commit(bar_s);
+    __syncthreads();                                     // P published, S read
+    if (is_p2) issue_pv(s & 1);
+    if (s + 1 < nsteps) {
+      mbar_wait(&full[(s + 1) & 1], ((s + 1) >> 1) & 1);
+      compute_s((s + 1) & 1);
     }
+    __syncthreads();
   }
-  mbar_wait(bar_s, nsteps & 1);
-  tc_fence_after();
 
   // ---- epilogue: O / l -> bf16, LSE ----
+  acc_store<64>(acc_s, 0, o[0]);
+  acc_store<64>(acc_s, 64, o[1]);
+  __syncthreads();
   const float inv_l = (l_run > 0.f) ? 1.0f / l_run : 0.f;
 #pragma unroll 1
   for (int c = 0; c < 2; ++c) {
     uint32_t r[32];
-    tmem_ld32(t_o + lane_addr + c * 32, r);
-    tmem_ld_wait();
+    acc_ld32<64>(acc_s, tid, c * 32, r);
     if (row_ok) {
       bf16* dst = p.out + static_cast<long long>(prob * p.Sq + row) * p.ldo + p.o_col0 + h * 64 + c * 32;
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
-        uint4 o;
-        o.x = pack_bf16x2(__uint_as_float(r[g * 8 + 0]) * inv_l, __uint_as_float(r[g * 8 + 1]) * inv_l);
-        o.y = pack_bf16x2(__uint_as_float(r[g * 8 + 2]) * inv_l, __uint_as_float(r[g * 8 + 3]) * inv_l);
-        o.z = pack_bf16x2(__uint_as_float(r[g * 8 + 4]) * inv_l, __uint_as_float(r[g * 8 + 5]) * inv_l);
-        o.w = pack_bf16x2(__uint_as_float(r[g * 8 + 6]) * inv_l, __uint_as_float(r[g * 8 + 7]) * inv_l);
-        *reinterpret_cast<uint4*>(dst + g * 8) = o;
+        uint4 ov;
+        ov.x = pack_bf16x2(__uint_as_float(r[g * 8 + 0]) * inv_l, __uint_as_float(r[g * 8 + 1]) * inv_l);
+        ov.y = pack_bf16x2(__uint_as_float(r[g * 8 + 2]) * inv_l, __uint_as_float(r[g * 8 + 3]) * inv_l);
+        ov.z = pack_bf16x2(__uint_as_float(r[g * 8 + 4]) * inv_l, __uint_as_float(r[g * 8 + 5]) * inv_l);
+        ov.w = pack_bf16x2(__uint_as_float(r[g * 8 + 6]) * inv_l, __uint_as_float(r[g * 8 + 7]) * inv_l);
+        *reinterpret_cast<uint4*>(dst + g * 8) = ov;
       }
     }
   }
   if (row_ok && p.lse != nullptr) {
     p.lse[(static_cast<long long>(prob) * p.H + h) * p.Sq + row] =
         (cls == 1 && l_run > 0.f) ? (m_run * p.scale + logf(l_run)) : 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 256);
-  }
-}
-
-// ================================================================================================
-// forward, S-resident variant (<= 3 key tiles = 384 keys: CLIP S=257, perceiver image 320, gated x-attn)
-//   All K/V tiles are TMA-loaded up front; every S_j = Q K_j^T stays in TMEM (128 columns per tile), so the
-//   softmax needs no second QK^T pass and no O rescaling.  256 threads: warps w and w+4 share TMEM lane
-//   quarter w%4 and split the 128 key columns of a tile in halves; row max / row sum are combined through smem.
-//   P tiles are double-buffered so softmax(tile j+1) overlaps the P V MMA of tile j.
-// ================================================================================================
-constexpr int kResThreads = 256;
-__global__ void __launch_bounds__(kResThreads)
-attn_fwd_resident_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv1,
-                         const __grid_constant__ CUtensorMap map_kv2, AttnParams p, int nt, int tmem_cols) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* s_q = smem;                              // 16 KB
-  uint8_t* s_k = s_q + kTileBytes;                  // nt x 16 KB
-  uint8_t* s_v = s_k + nt * kTileBytes;             // nt x 16 KB
-  uint8_t* s_p = s_v + nt * kTileBytes;             // 2 x 32 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_p + 4 * kTileBytes);
-  uint64_t* full_k = bars;          // [3]
-  uint64_t* full_v = bars + 3;      // [3]
-  uint64_t* bar_q = bars + 6;
-  uint64_t* bar_s = bars + 7;       // [3]
-  uint64_t* bar_pv = bars + 10;     // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
-  __shared__ float red[256];                          // [2][128] row partials
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qt = blockIdx.x, h = blockIdx.y, prob = blockIdx.z;
-  const int quarter = warp & 3, half = warp >> 2;
-  const int r_in_tile = quarter * 32 + lane;
-
-  if (tid == 32) {
-    for (int i = 0; i < 3; ++i) { mbar_init(&full_k[i], 1); mbar_init(&full_v[i], 1); mbar_init(&bar_s[i], 1); }
-    mbar_init(bar_q, 1); mbar_init(&bar_pv[0], 1); mbar_init(&bar_pv[1], 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  pdl_wait();   // predecessor grid complete before any global / TMA access
-  const uint32_t t_o = tmem + nt * 128;
-  const int nt1 = (p.Sk1 + 127) / 128;
-
-  const int row = qt * 128 + r_in_tile;
-  const bool row_ok = row < p.Sq;
-  int tt = 0;
-  if (p.text_time != nullptr && row_ok) tt = p.text_time[prob * p.Sq + row];
-  const int cls = row_ok ? row_class(p, tt) : 0;
-
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);
-  constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, false, true);
-
-  if (tid == 0) {
-    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_kv1); tma_prefetch_desc(&map_kv2);
-    mbar_arrive_expect_tx(bar_q, kTileBytes);
-    tma_load_2d(s_q, &map_q, bar_q, p.q_col0 + h * 64, prob * p.Sq + qt * 128);
-    for (int j = 0; j < nt; ++j) {
-      const KeyTile kt = key_tile(p, prob, j, nt1);
-      const CUtensorMap* m = kt.src ? &map_kv2 : &map_kv1;
-      mbar_arrive_expect_tx(&full_k[j], kTileBytes);
-      tma_load_2d(s_k + j * kTileBytes, m, &full_k[j], (kt.src ? p.k2_col0 : p.k1_col0) + h * 64, kt.row0);
-    }
-    for (int j = 0; j < nt; ++j) {
-      const KeyTile kt = key_tile(p, prob, j, nt1);
-      const CUtensorMap* m = kt.src ? &map_kv2 : &map_kv1;
-      mbar_arrive_expect_tx(&full_v[j], kTileBytes);
-      tma_load_2d(s_v + j * kTileBytes, m, &full_v[j], (kt.src ? p.v2_col0 : p.v1_col0) + h * 64, kt.row0);
-    }
-    mbar_wait(bar_q, 0);
-    const uint64_t da = make_smem_desc(smem_u32(s_q), 16, 1024);
-    for (int j = 0; j < nt; ++j) {
-      mbar_wait(&full_k[j], 0);
-      tc_fence_after();
-      const uint64_t db = make_smem_desc(smem_u32(s_k + j * kTileBytes), 16, 1024);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) umma_bf16(tmem + j * 128, da + k * 2, db + k * 2, idesc_s, k != 0);
-      umma_commit(&bar_s[j]);
-    }
-  }
-
-  const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-  // ---- sweep 1: row max over all resident tiles (this thread: 64 of the 128 columns of each tile) ----
-  float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-  for (int j = 0; j < nt; ++j) {
-    mbar_wait(&bar_s[j], 0);
-    tc_fence_after();
-    const KeyTile kt = key_tile(p, prob, j, nt1);
-    const RowRange rr = row_range(p, cls, tt, kt, row);
-    const bool whole = __all_sync(0xffffffffu, cls == 1 && rr.lo == 0 && rr.hi == 128);
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem + lane_addr + j * 128 + half * 64 + c * 32, r);
-      tmem_ld_wait();
-      if (whole) {
-#pragma unroll
-        for (int i = 0; i < 32; i += 4) {
-          mx[0] = fmaxf(mx[0], __uint_as_float(r[i]));     mx[1] = fmaxf(mx[1], __uint_as_float(r[i + 1]));
-          mx[2] = fmaxf(mx[2], __uint_as_float(r[i + 2])); mx[3] = fmaxf(mx[3], __uint_as_float(r[i + 3]));
-        }
-      } else if (cls == 1) {
-        const int c0 = half * 64 + c * 32;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int cc = c0 + i;
-          if (cc >= rr.lo && cc < rr.hi) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(r[i]));
-        }
-      }
-    }
-  }
-  float m_run = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-  red[half * 128 + r_in_tile] = m_run;
-  __syncthreads();
-  m_run = fmaxf(red[r_in_tile], red[128 + r_in_tile]);
-  __syncthreads();
-
-  // ---- sweep 2: P = exp2((S - m) * scale*log2e), O += P V ----
-  float ls[4] = {0.f, 0.f, 0.f, 0.f};
-  const float mb = (m_run == -INFINITY) ? 0.f : m_run * p.scale_log2;
-  for (int j = 0; j < nt; ++j) {
-    const KeyTile kt = key_tile(p, prob, j, nt1);
-    const RowRange rr = row_range(p, cls, tt, kt, row);
-    const bool whole = __all_sync(0xffffffffu, cls == 1 && rr.lo == 0 && rr.hi == 128);
-    uint8_t* pbuf = s_p + (j & 1) * 2 * kTileBytes;
-    if (j >= 2) mbar_wait(&bar_pv[j & 1], 0);          // P buffer (j-2) consumed
-#pragma unroll 1
-    for (int c = 0; c < 2; ++c) {
-      uint32_t r[32];
-      tmem_ld32(tmem + lane_addr + j * 128 + half * 64 + c * 32, r);
-      tmem_ld_wait();
-      float pv[32];
-      if (whole) {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          pv[i] = ex2_approx(fmaf(__uint_as_float(r[i]), p.scale_log2, -mb));
-          ls[i & 3] += pv[i];
-        }
-      } else {
-        const int c0 = half * 64 + c * 32;
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int cc = c0 + i;
-          float v = 0.f;
-          if (cc >= rr.lo && cc < rr.hi) v = (cls == 1) ? ex2_approx(fmaf(__uint_as_float(r[i]), p.scale_log2, -mb)) : 1.0f;
-          pv[i] = v;
-          ls[i & 3] += v;
-        }
-      }
-      uint8_t* chunk = pbuf + half * kTileBytes;       // 64-key chunk == this thread's column half
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint4 o;
-        o.x = pack_bf16x2(pv[g * 8 + 0], pv[g * 8 + 1]); o.y = pack_bf16x2(pv[g * 8 + 2], pv[g * 8 + 3]);
-        o.z = pack_bf16x2(pv[g * 8 + 4], pv[g * 8 + 5]); o.w = pack_bf16x2(pv[g * 8 + 6], pv[g * 8 + 7]);
-        st_sw128(chunk, r_in_tile, c * 32 + g * 8, o);
-      }
-    }
-    fence_proxy_async_smem();
-    tc_fence_before();
-    __syncthreads();
-    if (tid == 0) {
-      tc_fence_after();
-      mbar_wait(&full_v[j], 0);
-      tc_fence_after();
-      const uint64_t db = make_smem_desc(smem_u32(s_v + j * kTileBytes), 16, 1024);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) {
-        const uint64_t da = make_smem_desc(smem_u32(pbuf + (k >> 2) * kTileBytes) + (k & 3) * 32, 16, 1024);
-        umma_bf16(t_o, da, db + k * 128, idesc_pv, (j > 0 || k != 0) ? 1u : 0u);
-      }
-      umma_commit(&bar_pv[j & 1]);
-    }
-  }
-  float l_run = (ls[0] + ls[1]) + (ls[2] + ls[3]);
-  red[half * 128 + r_in_tile] = l_run;
-  // last P V must have retired before O is read: tile nt-1 is the (count)th completion of its barrier
-  {
-    const int jl = nt - 1;
-    mbar_wait(&bar_pv[jl & 1], (jl >> 1) & 1);
-    if (nt >= 2) { const int j2 = nt - 2; mbar_wait(&bar_pv[j2 & 1], (j2 >> 1) & 1); }
-  }
-  tc_fence_after();
-  __syncthreads();
-  l_run = red[r_in_tile] + red[128 + r_in_tile];
-  const float inv_l = (l_run > 0.f) ? 1.0f / l_run : 0.f;
-  {
-    uint32_t r[32];
-    tmem_ld32(t_o + lane_addr + half * 32, r);
-    tmem_ld_wait();
-    if (row_ok) {
-      bf16* dst = p.out + static_cast<long long>(prob * p.Sq + row) * p.ldo + p.o_col0 + h * 64 + half * 32;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        uint4 o;
-        o.x = pack_bf16x2(__uint_as_float(r[g * 8 + 0]) * inv_l, __uint_as_float(r[g * 8 + 1]) * inv_l);
-        o.y = pack_bf16x2(__uint_as_float(r[g * 8 + 2]) * inv_l, __uint_as_float(r[g * 8 + 3]) * inv_l);
-        o.z = pack_bf16x2(__uint_as_float(r[g * 8 + 4]) * inv_l, __uint_as_float(r[g * 8 + 5]) * inv_l);
-        o.w = pack_bf16x2(__uint_as_float(r[g * 8 + 6]) * inv_l, __uint_as_float(r[g * 8 + 7]) * inv_l);
-        *reinterpret_cast<uint4*>(dst + g * 8) = o;
-      }
-    }
-  }
-  if (half == 0 && row_ok && p.lse != nullptr) {
-    p.lse[(static_cast<long long>(prob) * p.H + h) * p.Sq + row] =
-        (cls == 1 && l_run > 0.f) ? (m_run * p.scale + logf(l_run)) : 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, tmem_cols);
-  }
-}
-
-// ================================================================================================
-// forward, warp-specialised resident variant (<= 3 key tiles): the default for CLIP (S = 257), the perceiver on
-// image features (320 keys) and the gated cross-attention (64 * T keys).
-//
-//   warp 0      TMA producer: Q tiles (double-buffered), then every K / V tile once — they stay resident in smem
-//               for all query tiles of this (problem, head), so CLIP reads K/V once instead of once per query tile
-//   warp 1      allocates TMEM; one lane issues every tcgen05.mma:  S_j = Q K_j^T for all key tiles of a query tile
-//               (N = the tile's key count rounded up to 16: a 1-key remainder tile costs one 16-wide MMA), then,
-//               once the softmax warps have published P, O = sum_j P_j V_j; O is double-buffered
-//   warps 2-9   softmax + epilogue: warp pair (w, w+4) shares TMEM lane quarter w % 4 (= rows) and splits each key
-//               tile's 16-column chunks even / odd; row max and row sum are exchanged inside the pair through smem
-//               and a 64-thread named barrier.  Every key tile has its own P buffer (bf16, SW128), so a query tile
-//               needs ONE hand-off to the MMA warp, and the epilogue of tile i is deferred until after the softmax
-//               of tile i+1: the P V latency of tile i and the S latency of tile i+2 hide behind softmax work.
-// Every hand-off is an mbarrier (TMA complete_tx, tcgen05.commit, or one arrive per softmax warp): there is no
-// __syncthreads between the prologue and the teardown.  (ncu, CLIP shape, first version with per-key-tile hand-offs:
-// 25 us, most warp samples in mbarrier waits — profiles/r02_ncu_attn.md.)
-// ================================================================================================
-constexpr int kWsThreads = 320;
-__global__ void __launch_bounds__(kWsThreads, 1)
-attn_fwd_ws_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv1,
-                   const __grid_constant__ CUtensorMap map_kv2, AttnParams p, int nt, int nq_per_cta, int tmem_cols) {
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* s_q = smem;                              // 2 x 16 KB
-  uint8_t* s_k = s_q + 2 * kTileBytes;              // nt x 16 KB
-  uint8_t* s_v = s_k + nt * kTileBytes;             // nt x 16 KB
-  uint8_t* s_p = s_v + nt * kTileBytes;             // nt x 32 KB
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_p + 2 * nt * kTileBytes);
-  uint64_t* bar_q = bars;             // [2] Q tile landed
-  uint64_t* bar_qfree = bars + 2;     // [2] S MMAs that read the Q buffer retired
-  uint64_t* full_k = bars + 4;        // [3]
-  uint64_t* full_v = bars + 7;        // [3]
-  uint64_t* bar_s = bars + 10;        //     every S_j of this query tile complete
-  uint64_t* bar_sfree = bars + 11;    //     softmax finished reading S of this query tile (8 warp arrivals)
-  uint64_t* p_ready = bars + 12;      //     every P_j of this query tile written (8 warp arrivals)
-  uint64_t* bar_o = bars + 13;        // [2] O buffer complete (= the P V MMAs of that query tile retired)
-  uint64_t* bar_ofree = bars + 15;    // [2] epilogue finished reading the O buffer (8 warp arrivals)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 17);
-  // row max / row sum exchange of a warp pair, [2 column halves][128 rows]; dynamic: static + dynamic smem share the
-  // 227 KB limit and the resident tiles take 224 KB of it
-  float* red = reinterpret_cast<float*>(bars + 18);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int h = blockIdx.y, prob = blockIdx.z;
-  const int nqt = (p.Sq + 127) / 128;
-  const int qt0 = blockIdx.x * nq_per_cta;
-  const int nq = min(nq_per_cta, nqt - qt0);
-  const int nt1 = (p.Sk1 + 127) / 128;
-
-  if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar_q[i], 1); mbar_init(&bar_qfree[i], 1); mbar_init(&bar_o[i], 1); mbar_init(&bar_ofree[i], 8);
-    }
-    for (int i = 0; i < 3; ++i) { mbar_init(&full_k[i], 1); mbar_init(&full_v[i], 1); }
-    mbar_init(bar_s, 1); mbar_init(bar_sfree, 8); mbar_init(p_ready, 8);
-    fence_mbar_init();
-    // the loads need no TMEM: start them before the CTA-wide prologue barrier
-    tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_kv1); tma_prefetch_desc(&map_kv2);
-    pdl_wait();   // predecessor grid complete before any global / TMA access
-    mbar_arrive_expect_tx(&bar_q[0], kTileBytes);
-    tma_load_2d(s_q, &map_q, &bar_q[0], p.q_col0 + h * 64, prob * p.Sq + qt0 * 128);
-    for (int j = 0; j < nt; ++j) {
-      const KeyTile kt = key_tile(p, prob, j, nt1);
-      const CUtensorMap* m = kt.src ? &map_kv2 : &map_kv1;
-      mbar_arrive_expect_tx(&full_k[j], kTileBytes);
-      tma_load_2d(s_k + j * kTileBytes, m, &full_k[j], (kt.src ? p.k2_col0 : p.k1_col0) + h * 64, kt.row0);
-    }
-    for (int j = 0; j < nt; ++j) {
-      const KeyTile kt = key_tile(p, prob, j, nt1);
-      const CUtensorMap* m = kt.src ? &map_kv2 : &map_kv1;
-      mbar_arrive_expect_tx(&full_v[j], kTileBytes);
-      tma_load_2d(s_v + j * kTileBytes, m, &full_v[j], (kt.src ? p.v2_col0 : p.v1_col0) + h * 64, kt.row0);
-    }
-  }
-  if (warp == 1) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  const uint32_t t_o = tmem + nt * 128;       // two 64-column O buffers
-
-  if (warp == 0) {
-    // ===================== TMA producer: the remaining Q tiles =====================
-    if (lane == 0) {
-      for (int it = 1; it < nq; ++it) {
-        const int qb = it & 1;
-        if (it >= 2) mbar_wait(&bar_qfree[qb], ((it >> 1) - 1) & 1);
-        mbar_arrive_expect_tx(&bar_q[qb], kTileBytes);
-        tma_load_2d(s_q + qb * kTileBytes, &map_q, &bar_q[qb], p.q_col0 + h * 64, prob * p.Sq + (qt0 + it) * 128);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (single thread) =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 64, false, true);
-      for (int it = 0; it < nq; ++it) {
-        const int qb = it & 1, ob = it & 1;
-        mbar_wait(&bar_q[qb], (it >> 1) & 1);
-        if (it > 0) mbar_wait(bar_sfree, (it - 1) & 1);
-        tc_fence_after();
-        const uint64_t da = make_smem_desc(smem_u32(s_q + qb * kTileBytes), 16, 1024);
-        for (int j = 0; j < nt; ++j) {
-          if (it == 0) { mbar_wait(&full_k[j], 0); tc_fence_after(); }
-          const KeyTile kt = key_tile(p, prob, j, nt1);
-          const int ncols = (kt.valid + 15) & ~15;
-          const uint32_t idesc_s = make_idesc_bf16(128, ncols, false, false);
-          const uint64_t db = make_smem_desc(smem_u32(s_k + j * kTileBytes), 16, 1024);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_bf16(tmem + j * 128, da + k * 2, db + k * 2, idesc_s, k != 0);
-        }
-        umma_commit(bar_s);
-        umma_commit(&bar_qfree[qb]);
-        mbar_wait(p_ready, it & 1);
-        if (it >= 2) mbar_wait(&bar_ofree[ob], ((it >> 1) - 1) & 1);
-        tc_fence_after();
-        for (int j = 0; j < nt; ++j) {
-          if (it == 0) { mbar_wait(&full_v[j], 0); tc_fence_after(); }
-          const KeyTile kt = key_tile(p, prob, j, nt1);
-          const int ksteps = (kt.valid + 15) >> 4;
-          const uint8_t* pbuf = s_p + j * 2 * kTileBytes;
-          const uint64_t db = make_smem_desc(smem_u32(s_v + j * kTileBytes), 16, 1024);
-          for (int k = 0; k < ksteps; ++k) {
-            const uint64_t dp = make_smem_desc(smem_u32(pbuf + (k >> 2) * kTileBytes) + (k & 3) * 32, 16, 1024);
-            umma_bf16(t_o + ob * 64, dp, db + k * 128, idesc_pv, (j > 0 || k != 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(&bar_o[ob]);
-      }
-    }
-  } else {
-    // ===================== softmax + epilogue warps =====================
-    const int quarter = warp & 3;                 // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;             // even / odd 16-column chunks
-    const int r_in_tile = quarter * 32 + lane;
-    const uint32_t lane_addr = static_cast<uint32_t>(quarter * 32) << 16;
-    pdl_wait();
-
-    // O / l -> bf16 (this warp: 32 of the 64 head columns) + LSE of one finished query tile
-    auto epilogue = [&](int t, int row, bool row_ok, bool active, int cls, float m_run, float l_run) {
-      const int ob = t & 1;
-      if (active) {
-        const float inv_l = (l_run > 0.f) ? 1.0f / l_run : 0.f;
-        uint32_t r[32];
-        tmem_ld32(t_o + ob * 64 + lane_addr + half * 32, r);
-        tmem_ld_wait();
-        if (row_ok) {
-          bf16* dst = p.out + static_cast<long long>(prob * p.Sq + row) * p.ldo + p.o_col0 + h * 64 + half * 32;
-#pragma unroll
-          for (int g4 = 0; g4 < 4; ++g4) {
-            uint4 o;
-            o.x = pack_bf16x2(__uint_as_float(r[g4 * 8 + 0]) * inv_l, __uint_as_float(r[g4 * 8 + 1]) * inv_l);
-            o.y = pack_bf16x2(__uint_as_float(r[g4 * 8 + 2]) * inv_l, __uint_as_float(r[g4 * 8 + 3]) * inv_l);
-            o.z = pack_bf16x2(__uint_as_float(r[g4 * 8 + 4]) * inv_l, __uint_as_float(r[g4 * 8 + 5]) * inv_l);
-            o.w = pack_bf16x2(__uint_as_float(r[g4 * 8 + 6]) * inv_l, __uint_as_float(r[g4 * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(dst + g4 * 8) = o;
-          }
-          if (half == 0 && p.lse != nullptr)
-            p.lse[(static_cast<long long>(prob) * p.H + h) * p.Sq + row] =
-                (cls == 1 && l_run > 0.f) ? (m_run * p.scale + logf(l_run)) : 0.f;
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bar_ofree[ob]);
-    };
-
-    int p_row = 0, p_cls = 0;                       // the previous query tile, whose epilogue is still owed
-    bool p_row_ok = false, p_active = false;
-    float p_m = 0.f, p_l = 0.f;
-    for (int it = 0; it < nq; ++it) {
-      const int qt = qt0 + it;
-      const int row = qt * 128 + r_in_tile;
-      const bool row_ok = row < p.Sq;
-      const bool warp_active = (qt * 128 + quarter * 32) < p.Sq;      // warp-uniform
-      int tt = 0;
-      if (p.text_time != nullptr && row_ok) tt = p.text_time[prob * p.Sq + row];
-      const int cls = row_ok ? row_class(p, tt) : 0;
-
-      // ---- sweep 1: row max over the resident S tiles ----
-      mbar_wait(bar_s, it & 1);
-      tc_fence_after();
-      float mx[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
-      if (warp_active) {                            // warp-uniform: tcgen05.ld is a warp-collective instruction
-        for (int j = 0; j < nt; ++j) {
-          const KeyTile kt = key_tile(p, prob, j, nt1);
-          const RowRange rr = row_range(p, cls, tt, kt, row);
-          const int nch = (kt.valid + 15) >> 4;
-          const int my = (nch - half + 1) >> 1;       // this warp's chunks half, half+2, ... (<= 4), warp-uniform
-#pragma unroll
-          for (int b2 = 0; b2 < 2; ++b2) {            // two chunks in flight per wait: TMEM round trips were the
-            if (2 * b2 < my) {                        // per-tile cost of the first version
-              uint32_t r[2][16];
-#pragma unroll
-              for (int u = 0; u < 2; ++u)
-                if (2 * b2 + u < my) tmem_ld16(tmem + lane_addr + j * 128 + (half + 2 * (2 * b2 + u)) * 16, r[u]);
-              tmem_ld_wait();
-              if (cls == 1) {                         // zeroed / uniform rows need no maximum
-#pragma unroll
-                for (int u = 0; u < 2; ++u) {
-                  if (2 * b2 + u < my) {
-                    const int c0 = (half + 2 * (2 * b2 + u)) * 16;
-                    if (c0 >= rr.lo && c0 + 16 <= rr.hi) {
-#pragma unroll
-                      for (int i = 0; i < 16; ++i) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(r[u][i]));
-                    } else {
-#pragma unroll
-                      for (int i = 0; i < 16; ++i)
-                        if (c0 + i >= rr.lo && c0 + i < rr.hi) mx[i & 3] = fmaxf(mx[i & 3], __uint_as_float(r[u][i]));
-                    }
-                  }
-                }
-              }
-            }
-            __syncwarp();
-          }
-          __syncwarp();
-        }
-      }
-      float m_run = fmaxf(fmaxf(mx[0], mx[1]), fmaxf(mx[2], mx[3]));
-      if (warp_active) {
-        red[half * 128 + r_in_tile] = m_run;
-        named_bar_sync(1 + quarter, 64);
-        m_run = fmaxf(m_run, red[(half ^ 1) * 128 + r_in_tile]);
-      }
-      // the P V MMAs of the previous query tile retired: the P buffers may be overwritten (and its O is complete)
-      if (it > 0) { mbar_wait(&bar_o[(it - 1) & 1], ((it - 1) >> 1) & 1); tc_fence_after(); }
-
-      // ---- sweep 2: P = exp2((S - m) * scale * log2 e) -> smem (bf16), row sums ----
-      float ls[4] = {0.f, 0.f, 0.f, 0.f};
-      const float mb = (m_run == -INFINITY) ? 0.f : m_run * p.scale_log2;
-      if (warp_active) {
-        for (int j = 0; j < nt; ++j) {
-          const KeyTile kt = key_tile(p, prob, j, nt1);
-          const RowRange rr = row_range(p, cls, tt, kt, row);
-          const int nch = (kt.valid + 15) >> 4;
-          uint8_t* pbuf = s_p + j * 2 * kTileBytes;
-          const int my = (nch - half + 1) >> 1;
-#pragma unroll
-          for (int b2 = 0; b2 < 2; ++b2) {
-            if (2 * b2 < my) {
-              uint32_t r[2][16];
-#pragma unroll
-              for (int u = 0; u < 2; ++u)
-                if (2 * b2 + u < my) tmem_ld16(tmem + lane_addr + j * 128 + (half + 2 * (2 * b2 + u)) * 16, r[u]);
-              tmem_ld_wait();
-#pragma unroll
-              for (int u = 0; u < 2; ++u) {
-                if (2 * b2 + u < my) {
-                  const int c = half + 2 * (2 * b2 + u), c0 = c * 16;
-                  float pv[16];
-                  if (cls == 1 && c0 >= rr.lo && c0 + 16 <= rr.hi) {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                      pv[i] = ex2_approx(fmaf(__uint_as_float(r[u][i]), p.scale_log2, -mb));
-                      ls[i & 3] += pv[i];
-                    }
-                  } else {
-#pragma unroll
-                    for (int i = 0; i < 16; ++i) {
-                      float v = 0.f;
-                      if (c0 + i >= rr.lo && c0 + i < rr.hi)
-                        v = (cls == 1) ? ex2_approx(fmaf(__uint_as_float(r[u][i]), p.scale_log2, -mb)) : 1.0f;
-                      pv[i] = v;
-                      ls[i & 3] += v;
-                    }
-                  }
-                  uint8_t* chunk = pbuf + (c >> 2) * kTileBytes;
-#pragma unroll
-                  for (int w2 = 0; w2 < 2; ++w2) {
-                    uint4 o;
-                    o.x = pack_bf16x2(pv[w2 * 8 + 0], pv[w2 * 8 + 1]); o.y = pack_bf16x2(pv[w2 * 8 + 2], pv[w2 * 8 + 3]);
-                    o.z = pack_bf16x2(pv[w2 * 8 + 4], pv[w2 * 8 + 5]); o.w = pack_bf16x2(pv[w2 * 8 + 6], pv[w2 * 8 + 7]);
-                    st_sw128(chunk, r_in_tile, (c & 3) * 16 + w2 * 8, o);
-                  }
-                }
-              }
-            }
-            __syncwarp();
-          }
-        }
-        fence_proxy_async_smem();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(p_ready); mbar_arrive(bar_sfree); }   // P published; S may be overwritten
-
-      float l_run = (ls[0] + ls[1]) + (ls[2] + ls[3]);
-      if (warp_active) {
-        named_bar_sync(1 + quarter, 64);              // both warps of the pair have read the row maxima
-        red[half * 128 + r_in_tile] = l_run;
-        named_bar_sync(1 + quarter, 64);
-        l_run += red[(half ^ 1) * 128 + r_in_tile];
-        named_bar_sync(1 + quarter, 64);              // ... and the row sums, before the next tile's maxima land
-      }
-      // ---- deferred epilogue of the previous query tile (its O was complete before sweep 2 started) ----
-      if (it > 0) epilogue(it - 1, p_row, p_row_ok, p_active, p_cls, p_m, p_l);
-      p_row = row; p_row_ok = row_ok; p_active = warp_active; p_cls = cls; p_m = m_run; p_l = l_run;
-    }
-    mbar_wait(&bar_o[(nq - 1) & 1], ((nq - 1) >> 1) & 1);
-    tc_fence_after();
-    epilogue(nq - 1, p_row, p_row_ok, p_active, p_cls, p_m, p_l);
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, tmem_cols);
   }
 }
 
@@ -759,36 +211,28 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
   uint8_t* s_do = s_q + kTileBytes;         // 16 KB  dO_i
   uint8_t* s_p = s_do + kTileBytes;         // 32 KB  P   [128 rows][128 keys] (2 chunks)
   uint8_t* s_ds = s_p + 2 * kTileBytes;     // 32 KB  dS * scale
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_ds + 2 * kTileBytes);
+  uint8_t* acc_s = s_ds + 2 * kTileBytes;   // 32 KB  S of one 64-key half [128][64] fp32; dQ, dV afterwards
+  uint8_t* acc_dp = acc_s + 2 * kTileBytes; // 32 KB  dP of the same half; dK afterwards
+  uint64_t* bars = reinterpret_cast<uint64_t*>(acc_dp + 2 * kTileBytes);
   uint64_t* bar_kv = bars;
   uint64_t* bar_qdo = bars + 1;
-  uint64_t* bar_mma = bars + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3);
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const int h = blockIdx.x, prob = blockIdx.y;
 
-  if (tid == 32) {
-    mbar_init(bar_kv, 1); mbar_init(bar_qdo, 1); mbar_init(bar_mma, 1);
+  if (tid == 0) {
+    mbar_init(bar_kv, 1); mbar_init(bar_qdo, 1);
     fence_mbar_init();
   }
-  if (warp == 0) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
   pdl_wait();   // predecessor grid complete before any global / TMA access
-  const uint32_t t_s = tmem, t_dp = tmem + 128, t_dv = tmem + 256, t_dk = tmem + 320, t_dq = tmem + 384;
-  const uint32_t lane_addr = static_cast<uint32_t>(warp * 32) << 16;
 
   const int nt1 = (p.Sk1 + 127) / 128, nt2 = (p.Sk2 + 127) / 128, nkt = nt1 + nt2;
   const int nqt = (p.Sq + 127) / 128;
+  const uint32_t a_q = smem_u32(s_q), a_k = smem_u32(s_k), a_v = smem_u32(s_v), a_do = smem_u32(s_do);
+  const uint32_t a_p = smem_u32(s_p), a_ds = smem_u32(s_ds);
 
-  constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, false, false);   // S, dP
-  constexpr uint32_t idesc_t = make_idesc_bf16(128, 64, true, true);      // dV = P^T dO, dK = dS^T Q
-  constexpr uint32_t idesc_dq = make_idesc_bf16(128, 64, false, true);    // dQ = dS K
-
-  uint32_t ph_kv = 0, ph_qdo = 0, ph_mma = 0;
+  uint32_t ph_kv = 0, ph_qdo = 0;
   if (tid == 0) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_do); tma_prefetch_desc(&map_kv1); tma_prefetch_desc(&map_kv2);
   }
@@ -801,6 +245,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       tma_load_2d(s_k, m, bar_kv, (kt.src ? p.k2_col0 : p.k1_col0) + h * 64, kt.row0);
       tma_load_2d(s_v, m, bar_kv, (kt.src ? p.v2_col0 : p.v1_col0) + h * 64, kt.row0);
     }
+    float dv[2][32], dk[2][32];   // dV_j, dK_j: key rows [64 h, 64 h + 64)
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) { dv[hh][i] = 0.f; dk[hh][i] = 0.f; }
     for (int i = 0; i < nqt; ++i) {
       const int row = i * 128 + tid;
       const bool row_ok = row < p.Sq;
@@ -832,94 +281,77 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       const RowRange rr = row_range(p, cls, tt, kt, row);
       const float lse_l2 = lse * 1.4426950408889634f;
 
-      if (tid == 0) {
-        if (i == 0) { mbar_wait(bar_kv, ph_kv); }
-        mbar_wait(bar_qdo, ph_qdo);
-        tc_fence_after();
-        const uint64_t dq_ = make_smem_desc(smem_u32(s_q), 16, 1024);
-        const uint64_t dk_ = make_smem_desc(smem_u32(s_k), 16, 1024);
-        const uint64_t ddo = make_smem_desc(smem_u32(s_do), 16, 1024);
-        const uint64_t dv_ = make_smem_desc(smem_u32(s_v), 16, 1024);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(t_s, dq_ + k * 2, dk_ + k * 2, idesc_s, k != 0);      // S = Q K^T
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16(t_dp, ddo + k * 2, dv_ + k * 2, idesc_s, k != 0);    // dP = dO V^T
-        umma_commit(bar_mma);
-      }
+      if (i == 0) mbar_wait(bar_kv, ph_kv);
+      mbar_wait(bar_qdo, ph_qdo);
       ph_qdo ^= 1;
-      mbar_wait(bar_mma, ph_mma);
-      ph_mma ^= 1;
-      tc_fence_after();
 
 #pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t rs[32], rp[32];
-        tmem_ld32(t_s + lane_addr + c * 32, rs);
-        tmem_ld32(t_dp + lane_addr + c * 32, rp);
-        tmem_ld_wait();
-        uint8_t* pchunk = s_p + (c >> 1) * kTileBytes;
-        uint8_t* dchunk = s_ds + (c >> 1) * kTileBytes;
+      for (int kh = 0; kh < 2; ++kh) {           // keys [64 kh, 64 kh + 64): S = Q K^T, dP = dO V^T
+        wg_mma_tile<64, 0, 0>(
+            acc_s, 4, [&](int hh, int k) { return make_smem_desc(a_q + hh * 8192 + k * 32, 16, 1024); },
+            [&](int k) { return make_smem_desc(a_k + kh * 8192 + k * 32, 16, 1024); });
+        wg_mma_tile<64, 0, 0>(
+            acc_dp, 4, [&](int hh, int k) { return make_smem_desc(a_do + hh * 8192 + k * 32, 16, 1024); },
+            [&](int k) { return make_smem_desc(a_v + kh * 8192 + k * 32, 16, 1024); });
+        __syncthreads();
+#pragma unroll 1
+        for (int c2 = 0; c2 < 2; ++c2) {
+          const int c = kh * 2 + c2;
+          uint32_t rs[32], rp[32];
+          acc_ld32<64>(acc_s, tid, c2 * 32, rs);
+          acc_ld32<64>(acc_dp, tid, c2 * 32, rp);
+          uint8_t* pchunk = s_p + kh * kTileBytes;
+          uint8_t* dchunk = s_ds + kh * kTileBytes;
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float pv[8], dv[8];
+          for (int g = 0; g < 4; ++g) {
+            float pv[8], dsv[8];
 #pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            const int cc = c * 32 + g * 8 + e;
-            float pr = 0.f, ds = 0.f;
-            if (cc >= rr.lo && cc < rr.hi) {
-              if (cls == 1) {
-                pr = ex2_approx(fmaf(__uint_as_float(rs[g * 8 + e]), p.scale_log2, -lse_l2));
-                ds = pr * (__uint_as_float(rp[g * 8 + e]) - delta) * p.scale;
-              } else {
-                pr = inv_cnt;
+            for (int e = 0; e < 8; ++e) {
+              const int cc = c * 32 + g * 8 + e;
+              float pr = 0.f, ds = 0.f;
+              if (cc >= rr.lo && cc < rr.hi) {
+                if (cls == 1) {
+                  pr = ex2_approx(fmaf(__uint_as_float(rs[g * 8 + e]), p.scale_log2, -lse_l2));
+                  ds = pr * (__uint_as_float(rp[g * 8 + e]) - delta) * p.scale;
+                } else {
+                  pr = inv_cnt;
+                }
               }
+              pv[e] = pr; dsv[e] = ds;
             }
-            pv[e] = pr; dv[e] = ds;
+            uint4 o;
+            o.x = pack_bf16x2(pv[0], pv[1]); o.y = pack_bf16x2(pv[2], pv[3]);
+            o.z = pack_bf16x2(pv[4], pv[5]); o.w = pack_bf16x2(pv[6], pv[7]);
+            st_sw128(pchunk, tid, c2 * 32 + g * 8, o);
+            o.x = pack_bf16x2(dsv[0], dsv[1]); o.y = pack_bf16x2(dsv[2], dsv[3]);
+            o.z = pack_bf16x2(dsv[4], dsv[5]); o.w = pack_bf16x2(dsv[6], dsv[7]);
+            st_sw128(dchunk, tid, c2 * 32 + g * 8, o);
           }
-          uint4 o;
-          o.x = pack_bf16x2(pv[0], pv[1]); o.y = pack_bf16x2(pv[2], pv[3]);
-          o.z = pack_bf16x2(pv[4], pv[5]); o.w = pack_bf16x2(pv[6], pv[7]);
-          st_sw128(pchunk, tid, (c & 1) * 32 + g * 8, o);
-          o.x = pack_bf16x2(dv[0], dv[1]); o.y = pack_bf16x2(dv[2], dv[3]);
-          o.z = pack_bf16x2(dv[4], dv[5]); o.w = pack_bf16x2(dv[6], dv[7]);
-          st_sw128(dchunk, tid, (c & 1) * 32 + g * 8, o);
         }
+        __syncthreads();                          // acc_s / acc_dp read before the next half overwrites them
       }
       fence_proxy_async_smem();
-      tc_fence_before();
       __syncthreads();
 
-      if (tid == 0) {
-        tc_fence_after();
-        const uint32_t acc = (i > 0) ? 1u : 0u;
-        // dV += P^T dO ; dK += dS^T Q      A MN-major: 2 chunks of 64 keys, LBO = chunk stride, k-step = 16 q rows
-        const uint64_t a_p = make_smem_desc(smem_u32(s_p), kTileBytes, 1024);
-        const uint64_t a_ds = make_smem_desc(smem_u32(s_ds), kTileBytes, 1024);
-        const uint64_t b_do = make_smem_desc(smem_u32(s_do), 16, 1024);
-        const uint64_t b_q = make_smem_desc(smem_u32(s_q), 16, 1024);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(t_dv, a_p + k * 128, b_do + k * 128, idesc_t, (acc || k != 0) ? 1u : 0u);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) umma_bf16(t_dk, a_ds + k * 128, b_q + k * 128, idesc_t, (acc || k != 0) ? 1u : 0u);
-        // dQ = dS K   A K-major over keys (2 chunks), B = K_j MN-major
-        const uint64_t b_k = make_smem_desc(smem_u32(s_k), 16, 1024);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          const uint64_t a = make_smem_desc(smem_u32(s_ds + (k >> 2) * kTileBytes) + (k & 3) * 32, 16, 1024);
-          umma_bf16(t_dq, a, b_k + k * 128, idesc_dq, k != 0);
-        }
-        umma_commit(bar_mma);
-      }
-      mbar_wait(bar_mma, ph_mma);
-      ph_mma ^= 1;
-      tc_fence_after();
+      // dV += P^T dO ; dK += dS^T Q      A MN-major: key half hh = chunk hh, k-step = 16 q rows; B MN-major
+      wg_mma_regs<64, 1, 1>(
+          dv, i > 0, 8, [&](int hh, int k) { return make_smem_desc(a_p + hh * kTileBytes + k * 2048, kTileBytes, 1024); },
+          [&](int k) { return make_smem_desc(a_do + k * 2048, 16, 1024); });
+      wg_mma_regs<64, 1, 1>(
+          dk, i > 0, 8, [&](int hh, int k) { return make_smem_desc(a_ds + hh * kTileBytes + k * 2048, kTileBytes, 1024); },
+          [&](int k) { return make_smem_desc(a_q + k * 2048, 16, 1024); });
+      // dQ = dS K   A K-major over keys (2 chunks), B = K_j MN-major
+      wg_mma_tile<64, 0, 1>(
+          acc_s, 8,
+          [&](int hh, int k) { return make_smem_desc(a_ds + (k >> 2) * kTileBytes + hh * 8192 + (k & 3) * 32, 16, 1024); },
+          [&](int k) { return make_smem_desc(a_k + k * 2048, 16, 1024); });
+      __syncthreads();
 
       // dQ tile: accumulate across key tiles through the fp32 workspace (same thread owns the same row)
 #pragma unroll 1
       for (int c = 0; c < 2; ++c) {
         uint32_t r[32];
-        tmem_ld32(t_dq + lane_addr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32<64>(acc_s, tid, c * 32, r);
         if (row_ok) {
           float v[32];
 #pragma unroll
@@ -948,12 +380,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
           }
         }
       }
-      tc_fence_before();
       __syncthreads();
     }
     ph_kv ^= 1;
 
-    // dV_j, dK_j complete: TMEM lane t = key t of this tile
+    // dV_j, dK_j complete: row t of the tiles = key t of this tile
+    acc_store<64>(acc_s, 0, dv[0]); acc_store<64>(acc_s, 64, dv[1]);
+    acc_store<64>(acc_dp, 0, dk[0]); acc_store<64>(acc_dp, 64, dk[1]);
+    __syncthreads();
     {
       const bool key_ok = tid < kt.valid;
       bf16* base = kt.src ? p.dkv2 : p.dkv1;
@@ -961,12 +395,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
       const int dkc = kt.src ? p.dk2_col0 : p.dk1_col0, dvc = kt.src ? p.dv2_col0 : p.dv1_col0;
 #pragma unroll 1
       for (int w = 0; w < 2; ++w) {      // 0: dV, 1: dK
-        const uint32_t t_src = w ? t_dk : t_dv;
+        uint8_t* src = w ? acc_dp : acc_s;
 #pragma unroll 1
         for (int c = 0; c < 2; ++c) {
           uint32_t r[32];
-          tmem_ld32(t_src + lane_addr + c * 32, r);
-          tmem_ld_wait();
+          acc_ld32<64>(src, tid, c * 32, r);
           if (key_ok) {
             bf16* dst = base + static_cast<long long>(kt.row0 + tid) * ld + (w ? dkc : dvc) + h * 64 + c * 32;
 #pragma unroll
@@ -982,17 +415,12 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant
         }
       }
     }
-    tc_fence_before();
     __syncthreads();
-  }
-  if (warp == 0) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
   }
 }
 
-constexpr int kAttnFwdSmem = 7 * kTileBytes + 1024 + 128;
-constexpr int kAttnBwdSmem = 8 * kTileBytes + 1024 + 128;
+constexpr int kAttnFwdSmem = 11 * kTileBytes + 1024 + 128;
+constexpr int kAttnBwdSmem = 12 * kTileBytes + 1024 + 128;
 
 }  // namespace otb
 
@@ -1039,33 +467,9 @@ extern "C" int otb_attn_fwd(const otb_attn_desc* d, void* stream) {
   else mk2 = mk1;
   if (rc) return rc;
   dim3 grid((d->Sq + 127) / 128, d->H, d->P);
-  const int nt = (d->Sk1 + 127) / 128 + (d->Sk2 + 127) / 128;
-  // warp-specialised kernel by default (validated r2c3: 13 kernel + 71 module tests; CLIP 32.5 -> 23.3 us, A 11.1 -> 9.8,
-  // B 7.3 -> 5.5 us in graph replay); OTB_ATTN_WS=0 selects the round-1 resident kernel
-  static const bool ws_on = [] { const char* v = getenv("OTB_ATTN_WS"); return !(v && v[0] == '0'); }();
-  if (nt <= 3 && ws_on) {
-    // one CTA keeps K/V resident for ALL query tiles of its (problem, head) when that already fills the chip
-    // (CLIP: 8 images x 16 heads = 128 CTAs, one wave); otherwise one query tile per CTA for more parallelism
-    const int nqt = (d->Sq + 127) / 128;
-    const int nq_per_cta = (d->P * d->H >= (sm_count() * 4) / 5) ? nqt : 1;
-    // Q x2, K/V resident, one 32 KB P buffer per key tile, + alignment slack + barriers and the 1 KB exchange array
-    // (nt = 3: 231,680 of the 232,448 bytes a CTA may have; the kernel declares no static shared memory)
-    const int smem = (2 + 4 * nt) * kTileBytes + 1024 + 1280;
-    OTB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_ws_kernel, (2 + 4 * 3) * kTileBytes + 1024 + 1280));
-    const int tmem_cols = (nt == 1) ? 256 : 512;            // nt x 128 (S) + 2 x 64 (O)
-    dim3 g((nqt + nq_per_cta - 1) / nq_per_cta, d->H, d->P);
-    OTB_CHECK_CUDA(launch_k(attn_fwd_ws_kernel, g, dim3(kWsThreads), smem, static_cast<cudaStream_t>(stream), mq, mk1,
-                            mk2, p, nt, nq_per_cta, tmem_cols));
-  } else if (nt <= 3) {
-    const int smem = (1 + 2 * nt + 4) * kTileBytes + 1024 + 2048;
-    OTB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_resident_kernel, (1 + 2 * 3 + 4) * kTileBytes + 1024 + 2048));
-    const int tmem_cols = (nt == 1) ? 256 : 512;
-    OTB_CHECK_CUDA(launch_k(attn_fwd_resident_kernel, dim3(grid), dim3(kResThreads), smem, static_cast<cudaStream_t>(stream), mq, mk1, mk2, p, nt,
-                                                                                             tmem_cols));
-  } else {
-    OTB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel, kAttnFwdSmem));
-    OTB_CHECK_CUDA(launch_k(attn_fwd_kernel, dim3(grid), dim3(kAttnThreads), kAttnFwdSmem, static_cast<cudaStream_t>(stream), mq, mk1, mk2, p));
-  }
+  OTB_CHECK_CUDA(ensure_dyn_smem(attn_fwd_kernel, kAttnFwdSmem));
+  OTB_CHECK_CUDA(launch_k(attn_fwd_kernel, grid, dim3(kAttnThreads), kAttnFwdSmem, static_cast<cudaStream_t>(stream), mq,
+                          mk1, mk2, p));
   count_launch();
   OTB_CHECK_CUDA(cudaGetLastError());
   return OTB_OK;

@@ -1,8 +1,8 @@
-// otter_b200 — common device-side building blocks for the sm_100a kernels.
+// otter_b200 — common device-side building blocks for the sm_90a (Hopper) kernels.
 //
-// Everything here is a thin inline-PTX wrapper: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (TMEM alloc / mma / commit / ld) and the shared-memory / instruction
-// descriptors the 5th-gen tensor cores consume.  No CUTLASS/CuTe dependency.
+// Everything here is a thin inline-PTX wrapper: mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma) with
+// its shared-memory descriptors, and the fp32 shared-memory accumulator tiles the attention kernels read row by row.
+// No CUTLASS/CuTe dependency.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -41,7 +41,7 @@ __device__ __forceinline__ bool elect_one() {
 
 // Programmatic dependent launch: every kernel lets its successor's CTAs start early (launch_dependents) and
 // itself waits for the complete predecessor grid (and its memory) right before the first global access, so
-// prologues (barrier init, TMEM alloc, descriptor prefetch, launch latency) overlap the predecessor's tail.
+// prologues (barrier init, descriptor prefetch, launch latency) overlap the predecessor's tail.
 // Both are no-ops when the kernel was not launched with the programmatic-serialization attribute.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -56,7 +56,7 @@ __device__ __forceinline__ void fence_mbar_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void fence_proxy_async_smem() {
-  // make generic-proxy smem writes visible to the async proxy (TMA store, tcgen05.mma operand reads)
+  // make generic-proxy smem writes visible to the async proxy (TMA store, wgmma operand reads)
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
@@ -79,17 +79,14 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a pipeline bug turns into a trap (CUDA error) after ~2 s instead of a hung GPU.
+// Bounded wait: a pipeline bug turns into a trap (CUDA error) after ~2 s instead of a hung GPU.  No printf here: a
+// function call between wgmma issue and wait makes ptxas serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (((++spins) & 0x3ff) == 0 && (clock64() - t0) > 4000000000LL) {
-      printf("otb: mbarrier wait timeout (block %d,%d thread %d parity %u)\n", blockIdx.x, blockIdx.y, threadIdx.x,
-             parity);
-      __trap();
-    }
+    if (((++spins) & 0x3ff) == 0 && (clock64() - t0) > 4000000000LL) __trap();
   }
 }
 
@@ -104,17 +101,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-      : "memory");
-}
-// Same, multicast to every CTA of the cluster named in cta_mask: data lands at the same CTA-relative smem
-// offset in each destination CTA and completes on the mbarrier at the same CTA-relative offset there.
-__device__ __forceinline__ void tma_load_2d_mcast(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1,
-                                                  uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-        "h"(cta_mask)
       : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c0, int c1) {
@@ -141,135 +127,158 @@ __device__ __forceinline__ void tma_store_wait_all() {
 }
 
 // ----------------------------------------------------------------------------------------------
-// tcgen05: TMEM allocation, fences, MMA, commit, load
+// wgmma: warpgroup MMA (4 warps, 128 threads), bf16 x bf16 -> fp32, accumulator in registers
 // ----------------------------------------------------------------------------------------------
-// Executed by ONE full warp. ncols: power of two in [32, 512].
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// D[64 x N] (+)= A[64 x 16] . B[16 x N] with both operands read from shared memory through descriptors.  TA / TB = 1:
+// the operand is MN-major (A stored [k][m], B stored [k][n]) — the transposed reads dgrad / wgrad / P V need, with no
+// transpose copy.  scale_d = 0 ignores the old accumulator (first k-step).  Every thread of the warpgroup executes it.
+template <int N, int TA, int TB>
+struct Wgmma;
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single thread issues.
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed.
-// (implicitly performs tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
+template <int TA, int TB>
+struct Wgmma<64, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, %35, %36;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
 
-// Same, arriving on the mbarrier at this CTA-relative offset in every CTA of cta_mask (cluster multicast).
-__device__ __forceinline__ void umma_commit_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-                   "r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
-}
-// ---- cta_group::2 (two SMs of a TPC cooperate on one 256-row MMA) ----
-__device__ __forceinline__ void tmem_alloc_2cta(uint32_t* smem_result, uint32_t ncols) {   // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// Issued by the leader CTA only: D (256 x N, 128 rows in each CTA's TMEM) (+)= A (128 rows from each CTA) * B
-// (N/2 rows from each CTA); descriptors hold CTA-relative smem offsets valid in both CTAs.
-__device__ __forceinline__ void umma_bf16_2cta(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                               uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2cta_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::
-                   "r"(smem_u32(bar)), "h"(cta_mask)
-               : "memory");
-}
-// TMA load whose completion bytes are credited to the LEADER CTA's mbarrier (peer bit 24 of the shared address
-// cleared), while the data lands in the issuing CTA's own shared memory.
-__device__ __forceinline__ void tma_load_2d_2cta(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar) & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
-}
-// arrive on the mbarrier at this CTA-relative address in CTA `target_rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t target_rank) {
-  asm volatile(
-      "{\n"
-      ".reg .b32 ra;\n"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n"
-      "}\n" ::"r"(smem_u32(bar)),
-      "r"(target_rank)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+template <int TA, int TB>
+struct Wgmma<128, TA, TB> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, %67, %68;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(da), "l"(db), "r"(scale_d), "n"(TA), "n"(TB));
+  }
+};
+
+// the accumulator registers are about to be read or written by wgmma (orders earlier register / smem accesses)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+// at most N committed groups of this warpgroup still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R>
+__device__ __forceinline__ void wgmma_keep(float (&d)[R]) {   // registers stay live across the asynchronous MMA
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns. Thread i gets lane (base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+// ----------------------------------------------------------------------------------------------
+// fp32 accumulator tiles in shared memory
+// ----------------------------------------------------------------------------------------------
+// The attention kernels keep the softmax and epilogue code "thread t owns row t": a warpgroup's m64 fragments are
+// stored to a [rows][N] fp32 tile and each thread reads its row back.  16 B units are XOR-swizzled with (row & 7), so
+// both the fragment stores (8 rows x 2 units per warp) and the row reads (a quarter-warp = 8 consecutive rows) are free
+// of bank conflicts.  N >= 32.
+template <int N>
+__device__ __forceinline__ float* acc_at(uint8_t* tile, int row, int col) {
+  return reinterpret_cast<float*>(tile + row * (N * 4) + ((((col >> 2) ^ (row & 7))) << 4) + (col & 3) * 4);
 }
-// TMEM -> registers: 32 lanes x 16 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+// wgmma fragment of m64nN (rows row0 .. row0+63 of the tile) <-> tile.  Thread t of the warpgroup holds rows
+// row0 + 16 (t/32) + (t%32)/4 (+8), columns 8 j + 2 (t%4) (+1).
+template <int N>
+__device__ __forceinline__ void acc_store(uint8_t* tile, int row0, const float (&d)[N / 2]) {
+  const int t = threadIdx.x & 127;
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    const int col = 8 * j + 2 * (t & 3);
+    *reinterpret_cast<float2*>(acc_at<N>(tile, r, col)) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc_at<N>(tile, r + 8, col)) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// 32 consecutive columns [col0, col0 + 32) of one row (col0 a multiple of 4); 16-column variant below
+template <int N>
+__device__ __forceinline__ void acc_ld32(uint8_t* tile, int row, int col0, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const float4 v = *reinterpret_cast<const float4*>(acc_at<N>(tile, row, col0 + 4 * k));
+    r[4 * k] = __float_as_uint(v.x); r[4 * k + 1] = __float_as_uint(v.y);
+    r[4 * k + 2] = __float_as_uint(v.z); r[4 * k + 3] = __float_as_uint(v.w);
+  }
+}
+template <int N>
+__device__ __forceinline__ void acc_ld16(uint8_t* tile, int row, int col0, uint32_t (&r)[16]) {
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float4 v = *reinterpret_cast<const float4*>(acc_at<N>(tile, row, col0 + 4 * k));
+    r[4 * k] = __float_as_uint(v.x); r[4 * k + 1] = __float_as_uint(v.y);
+    r[4 * k + 2] = __float_as_uint(v.z); r[4 * k + 3] = __float_as_uint(v.w);
+  }
+}
+
+// A 128-row product by one warpgroup: tile[128 x N] = sum_k A_k . B_k over `ksteps` k16 steps, as two m64 halves.
+// a(h, k) is the descriptor of rows [64 h, 64 h + 64) of A at k-step k, b(k) the one of B.  Operands must be resident
+// (and, if written by threads, fenced to the async proxy); the caller synchronises before reading the tile.
+template <int N, int TA, int TB, typename ADesc, typename BDesc>
+__device__ __forceinline__ void wg_mma_tile(uint8_t* tile, int ksteps, ADesc a, BDesc b) {
+#pragma unroll 1
+  for (int h = 0; h < 2; ++h) {
+    float d[N / 2];
+#pragma unroll
+    for (int i = 0; i < N / 2; ++i) d[i] = 0.f;
+    wgmma_keep(d);
+    wgmma_fence();
+#pragma unroll 1
+    for (int k = 0; k < ksteps; ++k) Wgmma<N, TA, TB>::mma(d, a(h, k), b(k), k != 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_keep(d);
+    acc_store<N>(tile, 64 * h, d);
+  }
+}
+// Same product accumulated into registers: d[h] holds rows [64 h, 64 h + 64) of an H x 64-row tile (accumulate = false
+// starts from zero).
+template <int N, int TA, int TB, int H, typename ADesc, typename BDesc>
+__device__ __forceinline__ void wg_mma_regs(float (&d)[H][N / 2], bool accumulate, int ksteps, ADesc a, BDesc b) {
+#pragma unroll
+  for (int h = 0; h < H; ++h) wgmma_keep(d[h]);
+  wgmma_fence();
+#pragma unroll
+  for (int h = 0; h < H; ++h)
+#pragma unroll 1
+    for (int k = 0; k < ksteps; ++k) Wgmma<N, TA, TB>::mma(d[h], a(h, k), b(k), (accumulate || k != 0) ? 1 : 0);
+  wgmma_commit();
+  wgmma_wait<0>();
+#pragma unroll
+  for (int h = 0; h < H; ++h) wgmma_keep(d[h]);
+}
 
 // ----------------------------------------------------------------------------------------------
 // Descriptors
 // ----------------------------------------------------------------------------------------------
-// Shared-memory matrix descriptor (SWIZZLE_128B, sm_100 "version 1").
+// wgmma shared-memory matrix descriptor, SWIZZLE_128B:
 //   bits [0,14)  start address >> 4        bits [16,30) leading byte offset >> 4
-//   bits [32,46) stride byte offset >> 4   bits [46,48) version = 1     bits [61,64) layout type (2 = SW128)
+//   bits [32,46) stride byte offset >> 4   bits [62,64) layout type (1 = SW128); base offset 0 (1024 B-aligned atoms)
 // K-major operand tile  [rows][64 bf16 = 128 B], 8-row swizzle atoms of 1024 B:
-//     SBO = 1024 (next 8-row group), LBO unused (1).  K-step of 16 elements = +32 B on the start address.
+//     SBO = 1024 (next 8-row group), LBO unused (1).  K-step of 16 elements = +32 B on the start address; rows 64..127
+//     of a 128-row tile start 8 KB further.
 // MN-major operand tile [chunk of 64 MN][k rows][128 B]:
 //     SBO = 1024 (next 8 k-rows), LBO = bytes between 64-element MN chunks. K-step of 16 = +16 rows = +2048 B.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
@@ -277,16 +286,8 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t 
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
-}
-// Instruction descriptor for kind::f16, BF16 x BF16 -> FP32.
-//   [4,6) c fmt = 1 (f32)  [7,10) a fmt = 1 (bf16)  [10,13) b fmt = 1  [15] a major  [16] b major
-//   [17,23) N >> 3   [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -299,8 +300,7 @@ __device__ __forceinline__ float gelu_erf_grad(float x) {
   return cdf + x * pdf;
 }
 // x * sigmoid(1.702 x).  The reciprocal is MUFU.RCP (1 ulp): an IEEE division costs ~20 instructions and a branch to a
-// slow path per element, and the bf16 result cannot tell the difference (ncu r02: the bias + quick-GELU epilogue of CLIP fc1
-// executed 5.4x the instructions of the plain one with 2 epilogue warps per scheduler to hide them).
+// slow path per element, and the bf16 result cannot tell the difference.
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));

@@ -1,9 +1,9 @@
 // otter_b200 — fp32-grade forward path (parity mode): meets the north star's 1e-3 rel / 1e-5 abs against the
-// reference's fp32 forward.  The dense contractions still run on the tcgen05 GEMM: each fp32 operand is split into
+// reference's fp32 forward.  The dense contractions still run on the wgmma GEMM: each fp32 operand is split into
 // three bf16 terms x = x0 + x1 + x2 (24 mantissa bits) and the six significant cross products
 //   x0y0 + x0y1 + x1y0 + x1y1 + x0y2 + x2y0
 // are evaluated as ONE bf16 GEMM over a 6x longer reduction dimension (operands concatenated along K by
-// otb_split3_concat), accumulated in fp32 in TMEM.  LayerNorm / softmax / attention run in fp32 on CUDA cores
+// otb_split3_concat), accumulated in fp32 registers.  LayerNorm / softmax / attention run in fp32 on CUDA cores
 // (they are < 0.1 % of the FLOPs).  Forward only; used by tests and by `otter_b200.precision("fp32")`.
 #include "otb_common.cuh"
 #include "otb_host.h"

@@ -1,6 +1,6 @@
-// otter_b200 — tcgen05 / TMA GEMM with fused epilogues (the >99.9 %-of-FLOPs kernel of the hot path).
+// otter_b200 — wgmma / TMA GEMM with fused epilogues (the >99.9 %-of-FLOPs kernel of the hot path).
 //
-//   D[M,N] = epilogue( A[M,K] . B[N,K]^T ),  bf16 operands, fp32 accumulation in TMEM.
+//   D[M,N] = epilogue( A[M,K] . B[N,K]^T ),  bf16 operands, fp32 accumulation in registers.
 //
 // Serves every nn.Linear on the path and its autograd dgrad / wgrad:
 //   forward  y  = x W^T      : A = x  [M][K]  K-major,  B = W  [N][K]  K-major
@@ -8,15 +8,13 @@
 //   wgrad    dW = dy^T x     : A = dy read MN-major,    B = x  read MN-major (reduction over tokens)
 // (reference: modeling_otter.py:139-148,164-184,253-256,284-288,340,363-370; clip.py:106-149)
 //
-// Structure (one CTA per SM, persistent over output tiles, 384 threads):
-//   warp 10  : TMA producer   — cp.async.bulk.tensor 128B-swizzled tiles into a kStages-deep smem ring
-//   warp 11  : MMA issuer     — one thread issues tcgen05.mma (128 x BN x 16), tcgen05.commit frees smem slots
-//                               (highest warp ids: the issue arbiter favours them over the math-heavy epilogue)
-//   warp 8   : TMEM allocator — 2 x BN fp32 columns (double-buffered accumulator)
-//   warps 0-7: epilogue       — tcgen05.ld 32 lanes x 32 columns (two warps per TMEM lane quarter, each half of
-//                               the tile's columns), global operands prefetched per chunk, fused
-//                               bias/GELU/gate/residual, 16 B stores
-// The accumulator double buffer lets the epilogue of tile i overlap the main loop of tile i+1.
+// Structure (one CTA per SM, persistent over 128 x 128 output tiles, 384 threads = 3 warpgroups):
+//   warpgroup 2 : TMA producer  — one thread streams 128B-swizzled A / B tiles into a 4-deep smem ring
+//   warpgroups 0, 1 : MMA + epilogue — each issues wgmma.m64n128k16 for its 64 rows (accumulator: 64 fp32 registers
+//                 per thread), then parks the fragments in a swizzled fp32 smem tile and runs the fused
+//                 bias/GELU/gate/residual epilogue with one thread per (row, column half): 16 B stores or a TMA store
+// Shared memory: 4 x 32 KB ring + 2 x 32 KB fp32 tiles + 32 KB TMA-store stage = 224 KB of the 227 KB an H100 CTA may
+// use; deeper rings or 256-wide tiles do not fit beside the fp32 tiles.
 #include <cstdlib>
 
 #include "otb_common.cuh"
@@ -25,10 +23,17 @@
 namespace otb {
 
 constexpr int kBM = 128;
+constexpr int kBN = 128;
 constexpr int kBK = 64;
-constexpr int kGemmThreads = 384;   // 8 epilogue warps + 4 control warps
+constexpr int kGemmThreads = 384;   // 2 MMA/epilogue warpgroups + 1 producer warpgroup
+constexpr int kStages = 4;
+constexpr int kABytes = kBM * kBK * 2;              // 16 KB
+constexpr int kBBytes = kBN * kBK * 2;              // 16 KB
+constexpr int kStageBytes = kABytes + kBBytes;
+constexpr int kAccBytes = 64 * kBN * 4;             // one warpgroup's 64 x 128 fp32 tile
 constexpr int kEpiWarpStage = 32 * 128;             // one epilogue warp's store stage: 32 rows x 128 B (64 bf16 columns)
-constexpr int kEpiStageBytes = 8 * kEpiWarpStage;    // 32 KB, sits between the operand ring and the barriers
+constexpr int kEpiStageBytes = 8 * kEpiWarpStage;   // 32 KB, sits between the fp32 tiles and the barriers
+constexpr int kGemmSmemBytes = kStages * kStageBytes + 2 * kAccBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 
 struct GemmEpi {
   const float* bias;
@@ -45,19 +50,10 @@ struct GemmEpi {
   int cls;        // index into kEpiCls when the options match one of the compiled classes, else -1 (run-time options)
 };
 
-template <int BN>
-struct GemmCfg {
-  static constexpr int kABytes = kBM * kBK * 2;            // 16 KB
-  static constexpr int kBBytes = BN * kBK * 2;             // 32 KB (BN=256) / 16 KB (BN=128)
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = (BN == 256) ? 4 : 6;
-  static constexpr int kTmemCols = 2 * BN;                 // double-buffered accumulator
-  static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
-};
 
-// One epilogue warp's share of one 128 x BN accumulator tile: TMEM lane quarter q (32 rows), column half `half`.
+// One epilogue warp's share of a warpgroup's 64 x BN accumulator tile `acc`: 32-row quarter q, column half `half`.
 template <int BN>
-__device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, uint32_t taddr, int m0, int n0, int M,
+__device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
                                               int N, int q, int half, int lane) {
   const int row = m0 + q * 32 + lane;
   const bool row_ok = row < M;
@@ -89,8 +85,7 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, ui
       }
     }
     uint32_t r[32];
-    tmem_ld32(taddr + c * 32, r);
-    tmem_ld_wait();
+    acc_ld32<BN>(acc, q * 32 + lane, c * 32, r);
     if (act_chunk) {
 #pragma unroll
       for (int g = 0; g < 4; ++g) {
@@ -177,12 +172,10 @@ __device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, ui
 // to the TMA engine, which writes whole lines, clips rows >= M / columns >= N, and for `accumulate` performs the
 // fp32 add at L2 (cp.reduce.async.bulk ... add) so the old values never travel to the SM.
 // The stage is reused once the previous bulk operation has finished READING it (wait_group.read), which overlaps
-// with the TMEM load and the math of the next chunk.  The pre-activation side output (aux_out) keeps direct stores.
+// with the accumulator read and the math of the next chunk.  The pre-activation side output (aux_out) keeps direct stores.
 // CLS >= 0: the epilogue options of launch class kEpiCls[CLS] are compile-time constants — the per-group option tests
 // (uniform branches that cut the 32 independent element streams of a chunk into tiny basic blocks) disappear and the
-// chunk becomes one block the scheduler can interleave.  ncu r02 (profiles/r02_ncu_gemm_epilogue.md): the generic code
-// executes 42 instructions per output for GELU + aux at 0.36 IPC per scheduler with 2 epilogue warps each; 29 % of the
-// stall samples sit on those branches.  CLS = -1: options read from `ep` at run time (any combination).
+// chunk becomes one block the scheduler can interleave.  CLS = -1: options read from `ep` at run time (any combination).
 struct EpiCls { bool bias, aux_out; int act; bool aux_in, scale, res, out_f32, acc; };
 constexpr int kNumEpiCls = 14;
 constexpr EpiCls kEpiCls[kNumEpiCls] = {
@@ -203,7 +196,7 @@ constexpr EpiCls kEpiCls[kNumEpiCls] = {
 };
 
 template <int BN, int CLS>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale, uint32_t taddr, int m0, int n0, int M,
+__device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
                                                   int N, int q, int half, int lane, uint8_t* stage,
                                                   const CUtensorMap* map_d) {
   constexpr bool kS = CLS >= 0;
@@ -242,8 +235,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
       }
     }
     uint32_t r[32];
-    tmem_ld32(taddr + c * 32, r);
-    tmem_ld_wait();
+    acc_ld32<BN>(acc, q * 32 + lane, c * 32, r);
     // bf16: two chunks share one 128 B-wide box (units 0-3 / 4-7); fp32: one chunk is one box (units 0-7).
     const bool first_of_box = f_f32 || (c & 1) == 0;
     const bool last_of_box = f_f32 || (c & 1) == 1 || colbase + 32 >= N;
@@ -333,192 +325,154 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
 
 // per-tile dispatch on the launch's epilogue class (host: epi_class_of)
 template <int BN>
-__device__ __forceinline__ void epilogue_dispatch_tma(const GemmEpi& ep, float scale, uint32_t taddr, int m0, int n0,
+__device__ __forceinline__ void epilogue_dispatch_tma(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0,
                                                       int M, int N, int q, int half, int lane, uint8_t* stage,
                                                       const CUtensorMap* map_d) {
-#define OTB_EPI_CASE(C_) case C_: epilogue_tile_tma<BN, C_>(ep, scale, taddr, m0, n0, M, N, q, half, lane, stage, map_d); break;
+#define OTB_EPI_CASE(C_) case C_: epilogue_tile_tma<BN, C_>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
   switch (ep.cls) {
     OTB_EPI_CASE(0) OTB_EPI_CASE(1) OTB_EPI_CASE(2) OTB_EPI_CASE(3) OTB_EPI_CASE(4) OTB_EPI_CASE(5) OTB_EPI_CASE(6)
     OTB_EPI_CASE(7) OTB_EPI_CASE(8) OTB_EPI_CASE(9) OTB_EPI_CASE(10) OTB_EPI_CASE(11) OTB_EPI_CASE(12) OTB_EPI_CASE(13)
-    default: epilogue_tile_tma<BN, -1>(ep, scale, taddr, m0, n0, M, N, q, half, lane, stage, map_d); break;
+    default: epilogue_tile_tma<BN, -1>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
   }
 #undef OTB_EPI_CASE
 }
 
-// MC = true: clusters of 2 CTAs work on two vertically adjacent 128-row tiles of the same BN-wide column block;
-// each CTA fetches half of the shared B tile and TMA-multicasts it to both, which cuts the L2->SM operand
-// traffic per FLOP by a third (the big GEMMs are L2-bandwidth bound at one 128xBN tile per CTA).
-template <int BN, bool A_MN, bool B_MN, bool MC, bool TS>
+// Persistent warp-specialised kernel, one CTA per SM.  Warpgroup 2 (one thread) is the TMA producer; warpgroups 0 and 1
+// each own 64 rows of the 128 x 128 tile: 4 wgmma.m64n128k16 per 64-deep k-block, one k-block kept in flight while the
+// next one issues (wait_group 1), its ring slot released as soon as the previous k-block's MMAs retire.  At the end of
+// a tile the warpgroup parks its fragments in its 32 KB fp32 tile and runs the epilogue row by row from there, while
+// the producer already streams the next tile's operands into the ring.
+template <bool A_MN, bool B_MN, bool TS>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_d, int M, int N, int K, GemmEpi ep) {
-  using Cfg = GemmCfg<BN>;
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_stage = smem + Cfg::kStages * Cfg::kStageBytes;      // 8 x 4 KB (1024-aligned), TMA-store epilogue only
+  uint8_t* acc_tiles = smem + kStages * kStageBytes;                 // 2 x 32 KB (one per MMA warpgroup)
+  uint8_t* epi_stage = acc_tiles + 2 * kAccBytes;                    // 8 x 4 KB (1024-aligned), TMA-store epilogue only
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + (TS ? kEpiStageBytes : 0));
   uint64_t* full_bar = bars;                        // [kStages]
-  uint64_t* empty_bar = bars + Cfg::kStages;        // [kStages]
-  uint64_t* tfull_bar = bars + 2 * Cfg::kStages;    // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;             // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
+  uint64_t* empty_bar = bars + kStages;             // [kStages]
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
-  const int tiles_m_real = (M + kBM - 1) / kBM;
-  const int tiles_m = MC ? ((tiles_m_real + 1) & ~1) : tiles_m_real;   // MC: pad to whole CTA pairs (OOB rows = 0)
-  const int tiles_n = (N + BN - 1) / BN;
+  const int tiles_m = (M + kBM - 1) / kBM;
+  const int tiles_n = (N + kBN - 1) / kBN;
   const int num_tiles = tiles_m * tiles_n;
   const int num_kb = (K + kBK - 1) / kBK;
-  const uint32_t cta_rank = MC ? cluster_ctarank() : 0;
-  // persistent schedule: consecutive tile ids run down M, so with MC the pair (2i, 2i+1) shares its column block;
-  // blockIdx.x of a cluster is (2c, 2c+1) and gridDim.x is even -> both CTAs walk the same number of tiles.
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
-    for (int s = 0; s < Cfg::kStages; ++s) {
+    for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], MC ? 2 : 1);   // MC: both CTAs of the pair must have consumed the stage
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 8);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[s], 2);   // one arrive per MMA warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  if constexpr (MC) cluster_sync_all();       // peer barriers are initialised before any multicast can land
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();   // predecessor grid complete before any global / TMA access
 
-  if (warp == 10 && lane == 0) {
+  if (wg == 2) {
     // ===================== TMA producer =====================
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int m0 = (t % tiles_m) * kBM;
-      const int n0 = (t / tiles_m) * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * Cfg::kStageBytes;
-        uint8_t* sb = sa + Cfg::kABytes;
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-        const int k0 = kb * kBK;
-        if constexpr (!A_MN) {
-          tma_load_2d(sa, &map_a, &full_bar[stage], k0, m0);  // box {64 k, 128 rows}
-        } else {
-#pragma unroll
-          for (int c = 0; c < kBM / 64; ++c)                  // box {64 m, 64 k rows} per 64-wide chunk
-            tma_load_2d(sa + c * (kBK * 128), &map_a, &full_bar[stage], m0 + c * 64, k0);
-        }
-        if constexpr (!MC) {
-          if constexpr (!B_MN) {
-            tma_load_2d(sb, &map_b, &full_bar[stage], k0, n0);  // box {64 k, BN rows}
+    if (threadIdx.x == 256) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        const int m0 = (t % tiles_m) * kBM;
+        const int n0 = (t / tiles_m) * kBN;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * kStageBytes;
+          uint8_t* sb = sa + kABytes;
+          mbar_arrive_expect_tx(&full_bar[stage], kStageBytes);
+          const int k0 = kb * kBK;
+          if constexpr (!A_MN) {
+            tma_load_2d(sa, &map_a, &full_bar[stage], k0, m0);  // box {64 k, 128 rows}
           } else {
 #pragma unroll
-            for (int c = 0; c < BN / 64; ++c)
+            for (int c = 0; c < kBM / 64; ++c)                  // box {64 m, 64 k rows} per 64-wide chunk
+              tma_load_2d(sa + c * (kBK * 128), &map_a, &full_bar[stage], m0 + c * 64, k0);
+          }
+          if constexpr (!B_MN) {
+            tma_load_2d(sb, &map_b, &full_bar[stage], k0, n0);  // box {64 k, 128 rows}
+          } else {
+#pragma unroll
+            for (int c = 0; c < kBN / 64; ++c)
               tma_load_2d(sb + c * (kBK * 128), &map_b, &full_bar[stage], n0 + c * 64, k0);
           }
-        } else {  // this CTA's half of the B tile, multicast into both CTAs of the pair
-          if constexpr (!B_MN) {
-            tma_load_2d_mcast(sb + cta_rank * (BN / 2) * 128, &map_b, &full_bar[stage], k0,
-                              n0 + cta_rank * (BN / 2), 0x3);  // box {64 k, BN/2 rows}
-          } else {
-#pragma unroll
-            for (int c = 0; c < BN / 128; ++c) {
-              const int cc = cta_rank * (BN / 128) + c;
-              tma_load_2d_mcast(sb + cc * (kBK * 128), &map_b, &full_bar[stage], n0 + cc * 64, k0, 0x3);
-            }
-          }
+          if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 11 && lane == 0) {
-    // ===================== MMA issuer (single thread) =====================
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, A_MN, B_MN);
-    constexpr uint32_t a_lbo = A_MN ? kBK * 128 : 16, a_sbo = 1024, a_kstep = A_MN ? 2048 : 32;
-    constexpr uint32_t b_lbo = B_MN ? kBK * 128 : 16, b_sbo = 1024, b_kstep = B_MN ? 2048 : 32;
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);  // epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * Cfg::kStageBytes);
-        const uint32_t sb = sa + Cfg::kABytes;
-        const uint64_t da = make_smem_desc(sa, a_lbo, a_sbo);
-        const uint64_t db = make_smem_desc(sb, b_lbo, b_sbo);
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) {
-          umma_bf16(d_tmem, da + ((k * a_kstep) >> 4), db + ((k * b_kstep) >> 4), idesc, (kb | k) != 0);
-        }
-        if constexpr (MC) umma_commit_mcast(&empty_bar[stage], 0x3);   // release the slot in BOTH CTAs
-        else umma_commit(&empty_bar[stage]);  // frees this smem slot once the MMAs above retire
-        if (++stage == Cfg::kStages) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(&tfull_bar[acc]);      // accumulator complete -> epilogue
-    }
-  } else if (warp < 8) {
-    // ===================== epilogue warps (8): warp w -> TMEM lane quarter w%4, column half w/4 =========
-    const int q = warp & 3;
-    const int half = warp >> 2;
+  } else {
+    // ===================== MMA + epilogue warpgroups: rows [64 wg, 64 wg + 64) of each tile =====================
+    constexpr uint32_t a_lbo = A_MN ? kBK * 128 : 16, a_kstep = A_MN ? 2048 : 32;
+    constexpr uint32_t b_lbo = B_MN ? kBK * 128 : 16, b_kstep = B_MN ? 2048 : 32;
+    // this warpgroup's 64 rows of A: 8 KB into a K-major tile, the second 64-wide chunk of an MN-major one
+    constexpr uint32_t a_rows = 64 * 128;
+    uint8_t* acc = acc_tiles + wg * kAccBytes;
+    const int q = warp & 1, half = (warp >> 1) & 1;      // epilogue: 32-row quarter of the 64 rows, column half
     float scale = ep.alpha;
     if (ep.scale_ptr != nullptr) {
       const float s = __ldg(ep.scale_ptr);
       scale *= ep.scale_tanh ? tanhf(s) : s;
     }
-    int it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const int m0 = (t % tiles_m) * kBM;
-      const int n0 = (t / tiles_m) * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
+      const int n0 = (t / tiles_m) * kBN;
+      float d[kBN / 2];
+#pragma unroll
+      for (int i = 0; i < kBN / 2; ++i) d[i] = 0.f;
+      int prev_stage = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+        const uint32_t sb = sa + kABytes;
+        const uint64_t da = make_smem_desc(sa + wg * a_rows, a_lbo, 1024);
+        const uint64_t db = make_smem_desc(sb, b_lbo, 1024);
+        wgmma_keep(d);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBK / 16; ++k)
+          Wgmma<kBN, A_MN, B_MN>::mma(d, da + ((k * a_kstep) >> 4), db + ((k * b_kstep) >> 4), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                 // the previous k-block's MMAs retired: its slot is free
+        wgmma_keep(d);
+        if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
+        prev_stage = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_keep(d);
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
+      acc_store<kBN>(acc, 0, d);
+      named_bar_sync(1 + wg, 128);
       if constexpr (TS)
-        epilogue_dispatch_tma<BN>(ep, scale, taddr, m0, n0, M, N, q, half, lane, epi_stage + warp * kEpiWarpStage, &map_d);
+        epilogue_dispatch_tma<kBN>(ep, scale, acc, m0 + 64 * wg, n0, M, N, q, half, lane, epi_stage + warp * kEpiWarpStage,
+                                   &map_d);
       else
-        epilogue_tile<BN>(ep, scale, taddr, m0, n0, M, N, q, half, lane);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+        epilogue_tile<kBN>(ep, scale, acc, m0 + 64 * wg, n0, M, N, q, half, lane);
+      named_bar_sync(1 + wg, 128);                      // the fp32 tile is read before the next tile overwrites it
     }
-    if (TS && lane == 0) tma_store_wait_read<0>();   // the stage must outlive the last bulk store's reads
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (MC) cluster_sync_all();       // no CTA leaves while its peer may still signal / write into it
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
+    if (TS && lane == 0) tma_store_wait_read<0>();     // the stage must outlive the last bulk store's reads
   }
 }
 
-template <int BN, bool A_MN, bool B_MN, bool MC, bool TS>
+template <bool A_MN, bool B_MN, bool TS>
 static int launch_gemm(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
                        const GemmEpi& ep, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
   CUtensorMap ma, mb;
   int rc;
   if (!A_MN) rc = make_tmap_bf16_2d(&ma, A, M, K, lda, kBM, 64);   // [M][K], box 128 rows x 64 k
   else       rc = make_tmap_bf16_2d(&ma, A, K, M, lda, kBK, 64);   // [K][M], box 64 k-rows x 64 m
   if (rc) return rc;
-  if (!B_MN) rc = make_tmap_bf16_2d(&mb, B, N, K, ldb, MC ? BN / 2 : BN, 64);
+  if (!B_MN) rc = make_tmap_bf16_2d(&mb, B, N, K, ldb, kBN, 64);
   else       rc = make_tmap_bf16_2d(&mb, B, K, N, ldb, kBK, 64);
   if (rc) return rc;
   CUtensorMap md = ma;                                               // placeholder when the direct epilogue is used
@@ -527,224 +481,24 @@ static int launch_gemm(const void* A, long long lda, const void* B, long long ld
                      : make_tmap_bf16_2d(&md, ep.out, M, N, ep.ld_out, 32, 64);
     if (rc) return rc;
   }
-  auto kern = gemm_bf16_kernel<BN, A_MN, B_MN, MC, TS>;
-  constexpr int smem_bytes = Cfg::kSmemBytes + (TS ? kEpiStageBytes : 0);
+  auto kern = gemm_bf16_kernel<A_MN, B_MN, TS>;
+  constexpr int smem_bytes = kGemmSmemBytes + (TS ? kEpiStageBytes : 0);
   OTB_CHECK_CUDA(ensure_dyn_smem(kern, smem_bytes));   // per (instantiation, device)
-  const int tiles_m = (M + kBM - 1) / kBM, tiles_n = (N + BN - 1) / BN;
+  const int tiles = ((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN);
   cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
+  cudaLaunchAttribute attr[1];
   int nattr = 0;
   if (pdl_enabled()) {
     attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[nattr].val.programmaticStreamSerializationAllowed = 1;
     ++nattr;
   }
-  if (MC) {
-    const int pairs = ((tiles_m + 1) / 2) * tiles_n;
-    const int max_pairs = sm_count() / 2;
-    cfg.gridDim = dim3(2 * (pairs < max_pairs ? pairs : max_pairs));
-    attr[nattr].id = cudaLaunchAttributeClusterDimension;
-    attr[nattr].val.clusterDim.x = 2; attr[nattr].val.clusterDim.y = 1; attr[nattr].val.clusterDim.z = 1;
-    ++nattr;
-  } else {
-    const int tiles = tiles_m * tiles_n;
-    cfg.gridDim = dim3(tiles < sm_count() ? tiles : sm_count());
-  }
+  cfg.gridDim = dim3(tiles < sm_count() ? tiles : sm_count());
   cfg.attrs = attr;
   cfg.numAttrs = nattr;
   cfg.blockDim = dim3(kGemmThreads);
   cfg.dynamicSmemBytes = smem_bytes;
   cfg.stream = stream;
-  OTB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, ma, mb, md, M, N, K, ep));
-  count_launch();
-  return OTB_OK;
-}
-
-
-// ================================================================================================
-// cta_group::2 variant: a CTA pair (two SMs) computes one 256 x 256 output tile with a single tcgen05.mma stream
-// issued by the leader.  Each CTA stages its own 128 rows of A and HALF of the B tile (128 of the 256 columns), so a
-// k-block costs 32 KB of smem traffic per SM instead of 48 KB — the 128 x 256 single-CTA kernel saturates the SM's
-// shared-memory bandwidth (TMA writes + tensor-core reads = 192 B/clk > 128 B/clk) at ~66 % tensor-pipe activity —
-// and the ring deepens to 6 stages.  Barrier protocol: TMA of both CTAs completes on the leader's `full`;
-// tcgen05.commit multicasts `empty` / `tmem_full` to both CTAs; both epilogues arrive on the leader's `tmem_empty`.
-// ================================================================================================
-constexpr int k2Stages = 6;
-constexpr int k2StageBytes = 2 * 128 * kBK * 2;   // A 16 KB + B-half 16 KB
-constexpr int k2SmemBytes = k2Stages * k2StageBytes + 1024 + 256;
-
-template <bool A_MN, bool B_MN, bool TS>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-gemm2_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-                  const __grid_constant__ CUtensorMap map_d, int M, int N, int K, GemmEpi ep) {
-  constexpr int BN = 256;
-  pdl_launch_dependents();
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* epi_stage = smem + k2Stages * k2StageBytes;              // 8 x 4 KB (1024-aligned), TMA-store epilogue only
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + (TS ? kEpiStageBytes : 0));
-  uint64_t* full_bar = bars;                    // [k2Stages]  (leader's copy is the live one)
-  uint64_t* empty_bar = bars + k2Stages;        // [k2Stages]  (both CTAs)
-  uint64_t* tfull_bar = bars + 2 * k2Stages;    // [2]         (both CTAs)
-  uint64_t* tempty_bar = tfull_bar + 2;         // [2]         (leader's copy is the live one)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const int tiles_mp = (M + 255) / 256;          // 256-row pair tiles
-  const int tiles_n = (N + BN - 1) / BN;
-  const int num_pt = tiles_mp * tiles_n;
-  const int num_kb = (K + kBK - 1) / kBK;
-  const int cluster_id = blockIdx.x >> 1, num_clusters = gridDim.x >> 1;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&map_a);
-    tma_prefetch_desc(&map_b);
-    for (int s = 0; s < k2Stages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 16); }   // 8 warps x 2 CTAs
-    fence_mbar_init();
-  }
-  if (warp == 8) tmem_alloc_2cta(tmem_slot, 512);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-
-  if (warp == 10 && lane == 0) {
-    // ===================== TMA producer (both CTAs) =====================
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int pt = cluster_id; pt < num_pt; pt += num_clusters) {
-      const int m0 = (pt % tiles_mp) * 256 + static_cast<int>(rank) * 128;
-      const int n0 = (pt / tiles_mp) * BN + static_cast<int>(rank) * 128;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sa = smem + stage * k2StageBytes;
-        uint8_t* sb = sa + 128 * kBK * 2;
-        if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * k2StageBytes);   // bytes of BOTH CTAs
-        const int k0 = kb * kBK;
-        if constexpr (!A_MN) {
-          tma_load_2d_2cta(sa, &map_a, &full_bar[stage], k0, m0);
-        } else {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) tma_load_2d_2cta(sa + c * (kBK * 128), &map_a, &full_bar[stage], m0 + c * 64, k0);
-        }
-        if constexpr (!B_MN) {
-          tma_load_2d_2cta(sb, &map_b, &full_bar[stage], k0, n0);
-        } else {
-#pragma unroll
-          for (int c = 0; c < 2; ++c) tma_load_2d_2cta(sb + c * (kBK * 128), &map_b, &full_bar[stage], n0 + c * 64, k0);
-        }
-        if (++stage == k2Stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 11 && lane == 0 && rank == 0) {
-    // ===================== MMA issuer (leader CTA, single thread) =====================
-    constexpr uint32_t idesc = make_idesc_bf16(256, BN, A_MN, B_MN);
-    constexpr uint32_t a_lbo = A_MN ? kBK * 128 : 16, a_kstep = A_MN ? 2048 : 32;
-    constexpr uint32_t b_lbo = B_MN ? kBK * 128 : 16, b_kstep = B_MN ? 2048 : 32;
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int pt = cluster_id; pt < num_pt; pt += num_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + acc * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + stage * k2StageBytes);
-        const uint32_t sb = sa + 128 * kBK * 2;
-        const uint64_t da = make_smem_desc(sa, a_lbo, 1024);
-        const uint64_t db = make_smem_desc(sb, b_lbo, 1024);
-#pragma unroll
-        for (int k = 0; k < kBK / 16; ++k)
-          umma_bf16_2cta(d_tmem, da + ((k * a_kstep) >> 4), db + ((k * b_kstep) >> 4), idesc, (kb | k) != 0);
-        umma_commit_2cta_mcast(&empty_bar[stage], 0x3);
-        if (++stage == k2Stages) { stage = 0; phase ^= 1; }
-      }
-      umma_commit_2cta_mcast(&tfull_bar[acc], 0x3);
-    }
-  } else if (warp < 8) {
-    // ===================== epilogue warps (both CTAs; each CTA owns its 128 rows) =====================
-    const int q = warp & 3, half = warp >> 2;
-    float scale = ep.alpha;
-    if (ep.scale_ptr != nullptr) {
-      const float s = __ldg(ep.scale_ptr);
-      scale *= ep.scale_tanh ? tanhf(s) : s;
-    }
-    int it = 0;
-    for (int pt = cluster_id; pt < num_pt; pt += num_clusters, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      const int m0 = (pt % tiles_mp) * 256 + static_cast<int>(rank) * 128;
-      const int n0 = (pt / tiles_mp) * BN;
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + acc * BN;
-      if constexpr (TS)
-        epilogue_dispatch_tma<BN>(ep, scale, taddr, m0, n0, M, N, q, half, lane, epi_stage + warp * kEpiWarpStage, &map_d);
-      else
-        epilogue_tile<BN>(ep, scale, taddr, m0, n0, M, N, q, half, lane);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(&tempty_bar[acc], 0);      // leader's barrier
-    }
-    if (TS && lane == 0) tma_store_wait_read<0>();   // the stage must outlive the last bulk store's reads
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, 512);
-  }
-}
-
-template <bool A_MN, bool B_MN, bool TS>
-static int launch_gemm2(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
-                        const GemmEpi& ep, cudaStream_t stream) {
-  CUtensorMap ma, mb;
-  int rc;
-  if (!A_MN) rc = make_tmap_bf16_2d(&ma, A, M, K, lda, 128, 64);
-  else       rc = make_tmap_bf16_2d(&ma, A, K, M, lda, kBK, 64);
-  if (rc) return rc;
-  if (!B_MN) rc = make_tmap_bf16_2d(&mb, B, N, K, ldb, 128, 64);
-  else       rc = make_tmap_bf16_2d(&mb, B, K, N, ldb, kBK, 64);
-  if (rc) return rc;
-  CUtensorMap md = ma;
-  if (TS) {
-    rc = ep.out_fp32 ? make_tmap_f32_2d(&md, ep.out, M, N, ep.ld_out, 32, 32)
-                     : make_tmap_bf16_2d(&md, ep.out, M, N, ep.ld_out, 32, 64);
-    if (rc) return rc;
-  }
-  auto kern = gemm2_bf16_kernel<A_MN, B_MN, TS>;
-  constexpr int smem_bytes = k2SmemBytes + (TS ? kEpiStageBytes : 0);
-  OTB_CHECK_CUDA(ensure_dyn_smem(kern, smem_bytes));
-  const int num_pt = ((M + 255) / 256) * ((N + 255) / 256);
-  const int max_clusters = sm_count() / 2;
-  cudaLaunchConfig_t cfg = {};
-  cudaLaunchAttribute attr[2];
-  int nattr = 0;
-  if (pdl_enabled()) {
-    attr[nattr].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[nattr].val.programmaticStreamSerializationAllowed = 1;
-    ++nattr;
-  }
-  attr[nattr].id = cudaLaunchAttributeClusterDimension;
-  attr[nattr].val.clusterDim.x = 2; attr[nattr].val.clusterDim.y = 1; attr[nattr].val.clusterDim.z = 1;
-  ++nattr;
-  cfg.gridDim = dim3(2 * (num_pt < max_clusters ? num_pt : max_clusters));
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem_bytes;
-  cfg.stream = stream;
-  cfg.attrs = attr;
-  cfg.numAttrs = nattr;
   OTB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, ma, mb, md, M, N, K, ep));
   count_launch();
   return OTB_OK;
@@ -782,8 +536,8 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
   ep.alpha = e->alpha;
   ep.res_fp32 = e->res_fp32;
   OTB_CHECK_ARG(!e->res_fp32 || e->out_fp32, "otb_gemm_bf16: fp32 residual requires fp32 output");
-  // Outputs leave through the smem-staged TMA-store / reduce-add epilogue (r02: FFN up GELU+aux 194 -> 164 us, fp32
-  // wgrad 206 -> 171 us, step +3 %; profiles/r02_gemm_selftest_bench.md).  OTB_GEMM_EPI_TMA=0 selects direct stores.
+  // Outputs leave through the smem-staged TMA-store / reduce-add epilogue (full 128 B lines, fp32 accumulate performed
+  // at L2).  OTB_GEMM_EPI_TMA=0 selects direct stores.
   static const bool epi_tma = [] { const char* v = getenv("OTB_GEMM_EPI_TMA"); return !(v && v[0] == '0'); }();
   ep.tma_out = (epi_tma && !e->res_fp32 && (reinterpret_cast<uintptr_t>(e->out) & 15) == 0 &&
                 (!e->out_fp32 || e->ld_out % 4 == 0)) ? 1 : 0;
@@ -804,57 +558,15 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
   if (cls_off) ep.cls = -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
-  // Tile-N choice: 256-wide tiles unless that leaves most SMs idle.  CTA-pair multicast (MC) when there are at
-  // least two row tiles and enough pairs to fill the chip (otherwise single CTAs spread wider).
-  const int tiles_m = (M + kBM - 1) / kBM;
-  const int tiles256 = tiles_m * ((N + 255) / 256);
-  const bool bn128 = (N <= 128) || (tiles256 < sm_count() && N > 128);
-  const int tiles = bn128 ? tiles_m * ((N + 127) / 128) : tiles256;
-  static const bool mc_off = (getenv("OTB_GEMM_NO_MCAST") != nullptr);
-  // OTB_GEMM_MC_MIN_TILES: smallest tile count that uses the 2-CTA multicast variant (default: one tile per SM).  CLIP
-  // out_proj / fc2 (136 tiles of 128x128, K up to 4096) are L2-bandwidth bound at 64 FLOP/B; sharing the B tile in a
-  // pair cuts their L2 traffic by a quarter.
-  static const int mc_min_tiles = [] { const char* v = getenv("OTB_GEMM_MC_MIN_TILES"); return v ? atoi(v) : 0; }();
-  const bool mc = !mc_off && tiles_m >= 2 && (tiles_m % 2 == 0 || tiles_m >= 9) &&
-                  tiles >= (mc_min_tiles > 0 ? mc_min_tiles : sm_count());
   const int sel = (a_mn_major ? 2 : 0) | (b_mn_major ? 1 : 0);
-  // cta_group::2 pair kernel for the large problems (>= one 256x256 pair tile per SM pair)
-  static const int two_cta = [] { const char* e = getenv("OTB_GEMM_2CTA"); return e ? atoi(e) : 1; }();
-  // (sending the 36-pair-tile CLIP out_proj / fc2 problems to the pair kernel was measured slower: profiles/r02_call1_knob_ab.md)
-  const int pair_tiles = ((M + 255) / 256) * ((N + 255) / 256);
-  const bool pair_ok = !bn128 && pair_tiles >= sm_count() / 2;
-  if (two_cta && pair_ok) {
-#define OTB_GEMM2_CASE(A_, B_)                                                        \
-  return ep.tma_out ? launch_gemm2<A_, B_, true>(A, lda, B, ldb, M, N, K, ep, st)     \
-                    : launch_gemm2<A_, B_, false>(A, lda, B, ldb, M, N, K, ep, st)
-    switch (sel) {
-      case 0: OTB_GEMM2_CASE(false, false);
-      case 1: OTB_GEMM2_CASE(false, true);
-      case 3: OTB_GEMM2_CASE(true, true);
-      default: break;
-    }
-#undef OTB_GEMM2_CASE
-  }
-#define OTB_GEMM_CASE(BN_, A_, B_)                                                                   \
-  if (ep.tma_out)                                                                                     \
-    return mc ? launch_gemm<BN_, A_, B_, true, true>(A, lda, B, ldb, M, N, K, ep, st)                 \
-              : launch_gemm<BN_, A_, B_, false, true>(A, lda, B, ldb, M, N, K, ep, st);               \
-  return mc ? launch_gemm<BN_, A_, B_, true, false>(A, lda, B, ldb, M, N, K, ep, st)                  \
-            : launch_gemm<BN_, A_, B_, false, false>(A, lda, B, ldb, M, N, K, ep, st)
-  if (bn128) {
-    switch (sel) {
-      case 0: OTB_GEMM_CASE(128, false, false);
-      case 1: OTB_GEMM_CASE(128, false, true);
-      case 3: OTB_GEMM_CASE(128, true, true);
-      default: break;
-    }
-  } else {
-    switch (sel) {
-      case 0: OTB_GEMM_CASE(256, false, false);
-      case 1: OTB_GEMM_CASE(256, false, true);
-      case 3: OTB_GEMM_CASE(256, true, true);
-      default: break;
-    }
+#define OTB_GEMM_CASE(A_, B_)                                                    \
+  return ep.tma_out ? launch_gemm<A_, B_, true>(A, lda, B, ldb, M, N, K, ep, st) \
+                    : launch_gemm<A_, B_, false>(A, lda, B, ldb, M, N, K, ep, st)
+  switch (sel) {
+    case 0: OTB_GEMM_CASE(false, false);
+    case 1: OTB_GEMM_CASE(false, true);
+    case 3: OTB_GEMM_CASE(true, true);
+    default: break;
   }
 #undef OTB_GEMM_CASE
   return set_error(OTB_ERR_UNSUPPORTED, "otb_gemm_bf16: layout (A MN-major, B K-major) not instantiated");

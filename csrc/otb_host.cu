@@ -129,10 +129,10 @@ constexpr int kMaxDevices = 64;
 int sm_count() {
   static std::atomic<int> cache[kMaxDevices];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return 132;
   int n = cache[dev].load(std::memory_order_relaxed);
   if (n == 0) {
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cache[dev].store(n, std::memory_order_relaxed);
   }
   return n;
@@ -158,7 +158,7 @@ cudaError_t ensure_dyn_smem(const void* func, int bytes) {
 extern "C" {
 const char* otb_last_error(void) { return otb::g_err; }
 int otb_version(void) { return 1; }
-int otb_compiled_arch(void) { return 100; }
+int otb_compiled_arch(void) { return 90; }
 long long otb_launch_count(void) { return otb::g_launches.load(); }
 long long otb_tmap_cache_stat(int which) { return which ? otb::g_tmap_misses.load() : otb::g_tmap_hits.load(); }
 int otb_abi_sizeof(int which) {

@@ -1,7 +1,7 @@
 // otter_b200 — LLaMA decoder-layer specific kernels (SURVEY.md §8f rank 1, the LLaMA-7B text model of OTTER-Video / c3).
 //   reference: xformers_model/llama.py:74-89 (LlamaRMSNorm), :150-166 (rotate_half / apply_rotary_pos_emb),
 //              :169-185 (LlamaMLP: down(silu(gate(x)) * up(x))), :186-259 (attention), :262-320 (decoder layer)
-// HBM-bound element-wise passes around the tcgen05 GEMMs and the head-dim-128 causal attention kernel:
+// HBM-bound element-wise passes around the wgmma GEMMs and the head-dim-128 causal attention kernel:
 //   rmsnorm fwd / bwd(dx)     y = x * rsqrt(mean(x^2) + eps) * w             (the LM is frozen: no weight gradient)
 //   rope (in place)           q, k columns of the [rows][3*D] projection buffer, rotate_half convention, head dim 128
 //   swiglu fwd / bwd          h = silu(g) * u ;  dg = dh * u * silu'(g), du = dh * silu(g)

@@ -253,7 +253,7 @@ extern "C" int otb_shifted_cross_entropy(const void* logits, int logits_fp32, in
 extern "C" int otb_scale_by_scalar(void* x, int x_fp32, int64_t n, const float* scalar, void* stream) {
   OTB_CHECK_ARG(x && scalar && n > 0, "otb_scale_by_scalar: bad argument");
   long long g = (n + 255) / 256;
-  if (g > 148 * 16) g = 148 * 16;
+  if (g > 132 * 16) g = 132 * 16;
   if (x_fp32)
     OTB_CHECK_CUDA(launch_k(scale_by_scalar_kernel<float>, dim3((unsigned)g), dim3(256), 0, ST(stream),
                             static_cast<float*>(x), (long long)n, scalar));

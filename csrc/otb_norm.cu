@@ -719,11 +719,11 @@ static int ln_fused_grid(int rows) {
 extern "C" int otb_ln_chunks(int rows, int D) {
   if (ln_fused_enabled() && D <= 4096) {        // workspace must hold one partial row per CTA of the one-pass kernel
     const int g = ln_fused_grid(rows);
-    int colblocks0 = (D + 63) / 64, chunks0 = (4 * 148 + colblocks0 - 1) / colblocks0;
+    int colblocks0 = (D + 63) / 64, chunks0 = (4 * 132 + colblocks0 - 1) / colblocks0;   // 4 x the H100's SMs
     return g > chunks0 ? g : chunks0;
   }
   int colblocks = (D + 63) / 64;
-  int chunks = (4 * 148 + colblocks - 1) / colblocks;
+  int chunks = (4 * 132 + colblocks - 1) / colblocks;
   if (chunks > (rows + 7) / 8) chunks = (rows + 7) / 8;
   if (chunks < 1) chunks = 1;
   return chunks;
@@ -736,7 +736,7 @@ extern "C" int otb_layernorm_bwd(const void* dy, int64_t lddy, const void* x, in
   OTB_CHECK_ARG(dy && x && mean && rstd && gamma && rows > 0 && D > 0, "otb_layernorm_bwd: bad argument");
   OTB_CHECK_ARG(D % 8 == 0 && lddy % 8 == 0 && ldx % 8 == 0, "otb_layernorm_bwd: D/ld must be multiples of 8");
   // dx == nullptr (perceiver norm_media: the frozen CLIP features need no input gradient) takes the one-pass kernel too:
-  // it then only produces the gamma / beta partials (r02 final launch list: the three-kernel fallback cost 34 us per call)
+  // it then only produces the gamma / beta partials, one launch instead of the three-kernel fallback
   if (ln_fused_enabled() && D <= 4096 && (dgamma != nullptr || dbeta != nullptr)) {
     OTB_CHECK_ARG((dx == nullptr || lddx % 8 == 0) && (add == nullptr || ldadd % 8 == 0), "otb_layernorm_bwd: bad ld");
     OTB_CHECK_ARG(ws != nullptr, "otb_layernorm_bwd: workspace required for parameter gradients");

@@ -220,7 +220,7 @@ int main(int argc, char** argv) {
       {128, 256, 64, 0, 1, 0},   {256, 512, 256, 0, 1, 0},   {200, 136, 200, 0, 1, 0},  {1000, 1024, 512, 0, 1, 3},
       {128, 256, 64, 1, 1, 0},   {256, 512, 256, 1, 1, 4},   {1024, 512, 1000, 1, 1, 4}, {2048, 4096, 300, 1, 1, 0},
       {4096, 4096, 1024, 0, 0, 0},
-      // CTA-pair multicast path (>= 148 tiles): odd row-tile count, all three layouts, heavy epilogues
+      // more tiles than SMs (persistent loop): odd row-tile count, all three layouts, heavy epilogues
       {2056, 4096, 1024, 0, 0, 5}, {2048, 16384, 512, 0, 1, 3}, {16384, 4096, 256, 1, 1, 4}, {2200, 4096, 320, 0, 0, 2},
       {2048, 16384, 320, 0, 0, 1}, {4096, 2560, 192, 1, 1, 0},
       // output-path coverage for the TMA-store epilogue: fp32 store with ragged M/N, bias + residual, N tail inside a box

@@ -1,4 +1,4 @@
-/* otter_b200 — C ABI of the B200-native vision-fusion hot path.
+/* otter_b200 — C ABI of the H100-native (sm_90a) vision-fusion hot path.
  *
  * The reference (Luodian/Otter) ships no native code and therefore has no FFI; the operations
  * below are the torch calls its hot-path modules make, restated as a C ABI so that a Python host
@@ -27,7 +27,7 @@ extern "C" {
 #define OTB_ERR_UNSUPPORTED 3
 
 const char* otb_last_error(void);
-/* Library/ABI version and the SM architecture the kernels were compiled for (100 = sm_100a). */
+/* Library/ABI version and the SM architecture the kernels were compiled for (90 = sm_90a). */
 int otb_version(void);
 int otb_compiled_arch(void);
 /* Number of kernels this library has launched in the calling process (bench.py "gpu_launches"). */
@@ -40,10 +40,10 @@ long long otb_tmap_cache_stat(int which);
 int otb_abi_sizeof(int which);
 
 /* ---------------------------------------------------------------------------------------------
- * GEMM:  D[M,N] = epilogue( A[M,K] . B[N,K]^T )      bf16 operands, fp32 accumulate in TMEM
+ * GEMM:  D[M,N] = epilogue( A[M,K] . B[N,K]^T )      bf16 operands, fp32 accumulate in registers
  * Replaces every nn.Linear / F.linear on the path (modeling_otter.py:139-148,164-167,180-184,
  * 253-256,284-288,340,363-370; xformers_model/clip.py:106-134,145-149) and their autograd
- * dgrad/wgrad.  tcgen05.mma + TMA, persistent, warp-specialised.
+ * dgrad/wgrad.  wgmma + TMA, persistent, warp-specialised.
  *
  * Operand layouts (ld* in elements):
  *   a_mn_major = 0 : A is stored [M][K] row-major (lda >= K)         (activations, dY for dgrad)
@@ -86,7 +86,7 @@ int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int
                   int N, int K, const otb_gemm_epilogue* epi, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Fused attention cores (tcgen05 QK^T / PV, online fp32 softmax, TMA-staged K/V tiles).
+ * Fused attention cores (wgmma QK^T / PV, two-sweep fp32 softmax, TMA-staged K/V tiles).
  *   (A) perceiver  latent x (vision ++ latents)   modeling_otter.py:168-179  (Sk2 > 0: second key source)
  *   (B) gated x-attn text x latents, media mask   modeling_otter.py:290-333  (text_time != NULL)
  *   (C) CLIP self-attention                       xformers_model/clip.py:112-128
@@ -164,7 +164,7 @@ typedef struct otb_lm_attn_desc {
 typedef struct otb_lm_attn_grads {
   const void* dout; /* [B*S][dout_cols] bf16, head h at dout_col0 + h*128 */
   void* dqkv;       /* [B*S][..] bf16: dQ / dK / dV of head h at dq_col0 / dk_col0 / dv_col0 + h*128 */
-  float* dq_ws;     /* fp32 [B*S][H*128] scratch, required when S > 128 */
+  float* dq_ws;     /* fp32 [B*S][H*128] scratch, required when S > 64 (the backward walks 64-key tiles) */
   int64_t ld_dout, ld_dqkv;
   int32_t dout_cols, dout_col0, dq_col0, dk_col0, dv_col0;
   int32_t _pad;

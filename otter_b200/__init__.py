@@ -1,7 +1,7 @@
-"""otter_b200 — B200-native (sm_100a) implementation of Otter's vision-fusion hot path.
+"""otter_b200 — H100-native (sm_90a) implementation of Otter's vision-fusion hot path.
 
 CLIP ViT patch encoder -> PerceiverResampler -> GatedCrossAttentionBlock, forward + backward, on
-hand-written tcgen05 / TMA CUDA kernels behind a C ABI (include/otter_b200.h), with the reference's
+hand-written wgmma / TMA CUDA kernels behind a C ABI (include/otter_b200.h), with the reference's
 module classes, forward() signatures and state-dict keys (otter_b200.modeling_otter).
 """
 __version__ = "0.1.0"

@@ -21,7 +21,7 @@ import os as _os
 
 # OTB_XATTN_FUSED=1: the gated block's attention + to_out + gate + residual run as ONE kernel (awaiting its GPU validation)
 XATTN_OUT_FUSED = _os.environ.get("OTB_XATTN_FUSED") == "1"
-WGRAD_SIDE_STREAM = False   # measured neutral on B200 (19.28 vs 19.31 ms/step): the large wgrads dominate
+WGRAD_SIDE_STREAM = False   # off: the large wgrads dominate the step, overlap has little to hide
 _side = {}
 
 

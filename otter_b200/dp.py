@@ -49,7 +49,7 @@ class FlatGradBuffer:
             raise ValueError("reduce_op must be 'sum' or 'avg'")
         # Wire-format collectives reduce with SUM and fold 1/world_size into the up-cast that follows: NCCL implements AVG
         # on floating types as pre-multiplied sum, which its in-switch (NVLS) algorithms do not take, so AVG pins the
-        # collective to RING (profiles/r02_scale_check_n4_n8.md).  'avg' keeps ncclAvg.
+        # collective to RING.  'avg' keeps ncclAvg.
         self.reduce_op = reduce_op
         direct_ids = {id(p) for p in (direct_params or [])}
         if direct_ids and (comm_dtype is None or comm_dtype == dtype):

@@ -2,7 +2,7 @@
 on the CUDA path itself, and — for the trainable perceiver / gated cross-attention blocks — its fp32 autograd gradients
 within 1e-3 as well.  Selected with `with otter_b200.precision("fp32"):`.
 
-Dense contractions run on the tcgen05 GEMM (three-term bf16 split, six cross products over a 6x longer reduction —
+Dense contractions run on the wgmma GEMM (three-term bf16 split, six cross products over a 6x longer reduction —
 functional.linear_f32; dgrad and wgrad go through the same routine on transposed operands); LayerNorm, softmax/attention,
 activation derivative, gate and row-bias gradients are fp32 CUDA-core kernels (csrc/otb_fp32.cu, csrc/otb_fp32_bwd.cu).
 Pure data movement (drop CLS, concat CLS token, im2col, transposes, broadcast of the latents) is torch indexing; autograd's

@@ -189,7 +189,7 @@ def lm_attn_bwd(dout, qkv, out, lse, B, S, H, *, slopes=None, causal=True, scale
     d = _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale)
     dqkv = torch.empty_like(qkv)
     g = LmAttnGrads()
-    ws = torch.empty((B * S, H * 128), device=qkv.device, dtype=torch.float32) if S > 128 else None
+    ws = torch.empty((B * S, H * 128), device=qkv.device, dtype=torch.float32) if S > 64 else None
     D = H * 128
     g.dout, g.dqkv, g.dq_ws = _p(dout), _p(dqkv), _p(ws)
     g.ld_dout, g.ld_dqkv = dout.stride(0), dqkv.stride(0)
@@ -616,8 +616,8 @@ def linear_f32(x, w6, N, *, bias=None, act=0, scale_ptr=None, scale_tanh=False, 
     out = torch.empty((M, N), device=x.device, dtype=torch.float32)
     if residual is not None:
         residual = _mat(residual, "residual", torch.float32)
-    # The tensor core adds into its fp32 accumulator with truncation, so a long in-TMEM reduction drifts by
-    # ~(#MMA steps) * 2^-24 of the running sum.  Keep each in-TMEM run short (F32_KCHUNK columns of K') and
+    # The tensor core adds into its fp32 accumulator with truncation, so a long in-accumulator reduction drifts by
+    # ~(#MMA steps) * 2^-24 of the running sum.  Keep each accumulator run short (F32_KCHUNK columns of K') and
     # carry the running sum in fp32 through the epilogue's round-to-nearest accumulate instead.
     K6, kc = 6 * K, F32_KCHUNK
     if K6 <= kc:

@@ -1,4 +1,4 @@
-"""Frozen MPT decoder layer on the otter_b200 kernels (SURVEY.md §8f rank 1; validated on the B200 in round 2).
+"""Frozen MPT decoder layer on the otter_b200 kernels (SURVEY.md §8f rank 1).
 
 Mirrors `MPTBlock` (/root/reference/src/otter_ai/models/mpt/blocks.py:23-88) — same sub-module and parameter names
 (`norm_1`, `attn.Wqkv`, `attn.out_proj`, `norm_2`, `ffn.up_proj`, `ffn.down_proj`), same `forward()` signature and

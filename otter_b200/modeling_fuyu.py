@@ -8,7 +8,7 @@ Mirrors /root/reference/src/otter_ai/models/fuyu/modeling_fuyu.py:
   * `embed_inputs(...)` — :122-131 (word embeddings + patches, skipped when `past_key_values` is given).
 The Persimmon language model itself is outside this path (SURVEY.md §8f rank 3).
 
-Arithmetic: the tcgen05 GEMM with the bias in its epilogue (K = 2700 is padded to 2704 = a 16-byte row pitch inside
+Arithmetic: the wgmma GEMM with the bias in its epilogue (K = 2700 is padded to 2704 = a 16-byte row pitch inside
 this module — callers pass the reference's shapes), then one scatter kernel (`otb_fuyu_scatter`) instead of the
 reference's per-sample `nonzero` + indexed copy.
 """

@@ -3,7 +3,7 @@
 Drop-in boundary (SURVEY.md §8b): same class names, constructor kwargs, forward() signatures, error
 behaviour and state-dict keys as /root/reference/src/otter_ai/models/otter/modeling_otter.py, so
 checkpoints load both ways and pipeline/train / pipeline/demos call sites work unchanged — but every
-forward/backward below runs on the sm_100a kernels of libotter_b200.so (via otter_b200.blocks).
+forward/backward below runs on the sm_90a kernels of libotter_b200.so (via otter_b200.blocks).
 There is no eager/PyTorch fallback: CPU tensors are rejected.
 
 Numerics: bf16 operands, fp32 accumulation / softmax / LayerNorm statistics — the reference's

@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in include/otter_b200.h but not exported"
     assert sorted(_lib.SIGNATURES) == syms, "ctypes SIGNATURES table out of sync with the header"
-    assert lib.otb_compiled_arch() == 100 and lib.otb_version() >= 1
+    assert lib.otb_compiled_arch() == 90 and lib.otb_version() >= 1
 
 
 def test_struct_layouts_match_header():
@@ -57,20 +57,19 @@ def test_ops_reject_cpu_tensors_loudly():
         F.linear_fwd(torch.zeros(8, 8, dtype=torch.bfloat16), torch.zeros(8, 8, dtype=torch.bfloat16))
 
 
-def test_sass_is_blackwell_native():
-    """The built library must contain 5th-gen tensor-core / TMA / TMEM machine code (B200_PROFILING.md:
-    tcgen05.mma -> UTC*MMA, TMA -> UTMALDG, tcgen05.ld -> LDTM) and no legacy mma.sync path (HMMA)."""
+def test_sass_is_hopper_native():
+    """The built library must contain sm_90a warpgroup tensor-core / TMA / mbarrier machine code (wgmma ->
+    HGMMA, TMA -> UTMALDG / UTMASTG, mbarrier -> SYNCS) and no legacy mma.sync path (HMMA)."""
     import shutil
     import subprocess
     from otter_b200 import _lib
     if shutil.which("cuobjdump") is None:
         pytest.skip("cuobjdump not on PATH")
     sass = subprocess.run(["cuobjdump", "-sass", _lib.LIB_PATH], capture_output=True, text=True, timeout=300).stdout
-    assert "sm_100a" in sass or "SM100" in sass.upper()
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UTCBAR", "SYNCS"):
+    assert "sm_90a" in sass
+    for mnemonic in ("HGMMA.64x128x16.F32.BF16", "HGMMA.64x64x16.F32.BF16", "UTMALDG", "UTMASTG", "SYNCS"):
         assert mnemonic in sass, f"{mnemonic} missing from the SASS"
-    assert "UTCHMMA.2CTA" in sass or "2CTA" in sass, "cta_group::2 MMA missing"
-    assert "HMMA." not in sass.replace("UTCHMMA", ""), "legacy mma.sync (HMMA) found"
+    assert "HMMA." not in sass, "legacy mma.sync (HMMA) found"
 
 
 def test_integration_guide_names_every_entry_point():

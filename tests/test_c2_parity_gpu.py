@@ -1,5 +1,5 @@
 """GPU: forward AND backward of the headline configuration (BASELINE.json configs[1]: D=4096, L=256, per-GPU batch 8)
-against the CPU oracle, plus the large-problem GEMM kernel (`gemm2_bf16_kernel`, cta_group::2) called directly
+against the CPU oracle, plus the GEMM kernel (`gemm_bf16_kernel`) called directly
 through the C ABI at the shapes / layouts / epilogues it runs with in the timed step.
 
 Tolerances are the production-mode (bf16 operands, fp32 accumulate) bounds of tests/test_modules_gpu.py, restated
@@ -72,7 +72,7 @@ def test_c2_gated_block_fwd_bwd_all_samples_vs_oracle():
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# gemm2_bf16_kernel at the step's own shapes (M = B*L = 2048 tokens, D = 4096, 4D = 16384), every FFN launch class
+# gemm_bf16_kernel at the step's own shapes (M = B*L = 2048 tokens, D = 4096, 4D = 16384), every FFN launch class
 # ---------------------------------------------------------------------------------------------------------------
 def _rn(g, *shape, scale=1.0):
     return (torch.randn(*shape, generator=g) * scale).to(BF16).to(DEV)

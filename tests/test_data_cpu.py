@@ -1,7 +1,7 @@
 """CPU: SURVEY.md §8f rank 4 — the oracle of the image transform is pinned against Pillow + torchvision themselves
 (the third-party arithmetic the reference calls: mimicit_dataset.py:132-143), the coefficient tables the CUDA kernels
-consume equal the oracle's, and the host-side collate / checkpoint helpers equal the reference's own functions
-(extracted verbatim by AST from the reference files)."""
+consume equal the oracle's, and the host-side collate / checkpoint helpers equal what the reference's own functions
+return (stored outputs)."""
 import os
 
 import numpy as np
@@ -9,7 +9,6 @@ import pytest
 import torch
 
 from oracle import preprocess as PP
-from oracle import ref_shims
 
 SIZES = [(480, 640), (224, 224), (100, 333), (1000, 750), (37, 41), (225, 223), (64, 2048)]
 
@@ -43,25 +42,17 @@ def test_kernel_coefficient_tables_equal_the_oracle():
     assert D.FLAMINGO_MEAN == PP.FLAMINGO_MEAN and D.FLAMINGO_STD == PP.FLAMINGO_STD
 
 
-@pytest.mark.skipif(not ref_shims.reference_available(), reason="needs /root/reference or oracle/_ref (build())")
 def test_collate_and_checkpoint_helpers_equal_the_reference_functions():
-    from oracle.make_golden_r2 import reference_function
+    """Outputs of the reference's own collate_tokens / get_checkpoint on the same inputs: tests/golden/reference_helpers.pt,
+    made by oracle/make_golden_live.py."""
+    from oracle.make_golden_live import COLLATE_CASES, checkpoint_module, collate_inputs
     from otter_b200 import checkpoint as CK
     from otter_b200 import data as D
-    ns = {"torch": torch}
-    exec(compile(reference_function("pipeline/mimicit_utils/mimicit_dataset.py", "collate_tokens"), "ref_collate", "exec"), ns)
-    g = torch.Generator().manual_seed(0)
-    for kw in (dict(pad_idx=1), dict(pad_idx=1, pad_to_length=40), dict(pad_idx=0, left_pad=True),
-               dict(pad_idx=None, eos_idx=2), dict(pad_idx=1, eos_idx=2, move_eos_to_beginning=True),
-               dict(pad_idx=1, pad_to_multiple=8)):
-        vals = [torch.randint(3, 50, (int(n),), generator=g) for n in torch.randint(1, 33, (5,), generator=g)]
-        assert torch.equal(ns["collate_tokens"](vals, **kw), D.collate_tokens(vals, **kw)), kw
-    ns2 = {"torch": torch}
-    exec(compile(reference_function("pipeline/train/train_utils.py", "get_checkpoint"), "ref_ckpt", "exec"), ns2)
-    m = torch.nn.Sequential(torch.nn.Linear(4, 4), torch.nn.LayerNorm(4), torch.nn.Linear(4, 2))
-    m[0].requires_grad_(False)
-    a, b = ns2["get_checkpoint"](m), CK.get_checkpoint(m)
-    assert list(a) == list(b) == ["1.weight", "1.bias", "2.weight", "2.bias"]
+    g = torch.load(os.path.join(os.path.dirname(__file__), "golden", "reference_helpers.pt"), weights_only=False)
+    for vals, kw, want in zip(collate_inputs(), COLLATE_CASES, g["collate"]):
+        assert torch.equal(want, D.collate_tokens(vals, **kw)), kw
+    b = CK.get_checkpoint(checkpoint_module())
+    assert g["checkpoint_keys"] == list(b) == ["1.weight", "1.bias", "2.weight", "2.bias"]
     assert D.resample_frames_fn(list(range(37)), 8) == [list(range(37))[i] for i in np.linspace(0, 36, 8, dtype=int)]
 
 

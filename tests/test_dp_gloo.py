@@ -175,7 +175,7 @@ def test_flat_allreduce_world2_bf16_direct_sinks():
 
 def test_reduce_op_argument():
     """The wire-format collective reduces with SUM (1/world_size folded into the up-cast) by default; 'avg' keeps ncclAvg;
-    anything else is rejected.  (On gloo both arms are SUM + divide — the NCCL arms are measured in profiles/r02_reduce_op_n4.md.)"""
+    anything else is rejected.  (On gloo both arms are SUM + divide.)"""
     import pytest
     from otter_b200.dp import FlatGradBuffer
     lin = torch.nn.Linear(8, 8)

@@ -1,7 +1,8 @@
 """CPU: the ALGORITHM csrc/otb_attn_lm.cu implements (log2-domain two-sweep softmax with the ALiBi key bias folded into
-the exponent, causal per-row key ranges per 128-key tile, LSE hand-over to the backward, dS = P (dP - delta) scale,
-dQ accumulated across key tiles) restated in numpy and checked against autograd of the reference-pinned oracle.
-It validates the formulas of the kernel — tile loop bounds, bias offsets, log domains — not the tcgen05 plumbing."""
+the exponent, causal per-row key ranges per key tile (128 keys forward, 64 backward), LSE hand-over to the backward,
+dS = P (dP - delta) scale, dQ accumulated across key tiles) restated in numpy and checked against autograd of the
+reference-pinned oracle.  It validates the formulas of the kernel — tile loop bounds, bias offsets, log domains — not the
+wgmma plumbing."""
 import math
 
 import numpy as np
@@ -12,9 +13,9 @@ from oracle import restatement_lm as R
 LOG2E = 1.4426950408889634
 
 
-def _row_hi(S, causal, row, j):
-    valid = min(128, S - j * 128)
-    return max(0, min(valid, row - j * 128 + 1)) if causal else valid
+def _row_hi(S, causal, row, k0, tk=128):
+    valid = min(tk, S - k0)
+    return max(0, min(valid, row - k0 + 1)) if causal else valid
 
 
 def kernel_algorithm(q, k, v, dout, slope, causal):
@@ -31,7 +32,7 @@ def kernel_algorithm(q, k, v, dout, slope, causal):
             m, l, acc = -np.inf, np.float32(0), np.zeros(128, np.float32)
             for sweep in (0, 1):
                 for j in range(nt):
-                    hi = _row_hi(S, causal, row, j)
+                    hi = _row_hi(S, causal, row, j * 128)
                     kf0 = np.float32(j * 128 - (S - 1))
                     for cc in range(hi):
                         s = np.float32(q[row] @ k[j * 128 + cc])
@@ -46,13 +47,14 @@ def kernel_algorithm(q, k, v, dout, slope, causal):
             lse[row] = (m + math.log2(l)) * 0.6931471805599453
     dq, dk, dv = np.zeros_like(q), np.zeros_like(k), np.zeros_like(v)
     delta = (dout * out).sum(1)
-    for j in range(nt_all):
-        for i in range(j if causal else 0, nt_all):
+    for j in range((S + 63) // 64):                      # backward: 64-key tiles, query tiles of 128 rows
+        k0 = j * 64
+        for i in range(k0 // 128 if causal else 0, nt_all):
             for row in range(i * 128, min(S, i * 128 + 128)):
-                hi = _row_hi(S, causal, row, j)
-                kf0 = np.float32(j * 128 - (S - 1))
+                hi = _row_hi(S, causal, row, k0, 64)
+                kf0 = np.float32(k0 - (S - 1))
                 for cc in range(hi):
-                    key = j * 128 + cc
+                    key = k0 + cc
                     t = np.float32(q[row] @ k[key]) * scale_log2 + slope2 * (kf0 + np.float32(cc))
                     pr = np.float32(2.0 ** (t - lse[row] * LOG2E))
                     dp = np.float32(dout[row] @ v[key])

@@ -1,4 +1,4 @@
-"""Developer tool: error of the fp32-grade split GEMM vs fp64 for several in-TMEM reduction lengths."""
+"""Developer tool: error of the fp32-grade split GEMM vs fp64 for several accumulator run lengths."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
