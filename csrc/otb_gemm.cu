@@ -8,13 +8,19 @@
 //   wgrad    dW = dy^T x     : A = dy read MN-major,    B = x  read MN-major (reduction over tokens)
 // (reference: modeling_otter.py:139-148,164-184,253-256,284-288,340,363-370; clip.py:106-149)
 //
-// Structure (one CTA per SM, persistent over 128 x 128 output tiles, 384 threads = 3 warpgroups):
-//   warpgroup 2 : TMA producer  — one thread streams 128B-swizzled A / B tiles into a 4-deep smem ring
-//   warpgroups 0, 1 : MMA + epilogue — each issues wgmma.m64n128k16 for its 64 rows (accumulator: 64 fp32 registers
-//                 per thread), then parks the fragments in a swizzled fp32 smem tile and runs the fused
-//                 bias/GELU/gate/residual epilogue with one thread per (row, column half): 16 B stores or a TMA store
-// Shared memory: 4 x 32 KB ring + 2 x 32 KB fp32 tiles + 32 KB TMA-store stage = 224 KB of the 227 KB an H100 CTA may
-// use; deeper rings or 256-wide tiles do not fit beside the fp32 tiles.
+// Structure (one CTA per SM, persistent over 128 x 128 output tiles, 384 threads = 3 warpgroups), ping-pong:
+//   warpgroup 2 : TMA producer  — one thread streams 128B-swizzled A / B tiles of the CTA's tiles, in order, into a
+//                 4-deep smem ring (register budget lowered to 40 with setmaxnreg)
+//   warpgroups 0, 1 : MMA + epilogue — they take alternate tiles of the CTA's sequence.  Each owns a whole 128 x 128
+//                 tile: two wgmma.m64n128k16 per k16 step, 128 fp32 accumulator registers per thread (budget raised to
+//                 232).  While one warpgroup runs its mainloop, the other runs the epilogue of its previous tile, so
+//                 the tensor cores do not wait for epilogues.  The epilogue parks the whole accumulator in a swizzled
+//                 fp32 smem tile shared by both warpgroups (their epilogues take turns) and runs the fused
+//                 bias/GELU/gate/residual epilogue with one thread per (row, column half): 16 B stores or a TMA store.
+// Tiles are walked in groups of 32 M-tiles (tile_origin) so one wave's operands stay in L2.
+// Shared memory: 4 x 32 KB ring + 64 KB fp32 park tile + 32 KB TMA-store stage = 224 KB of the 227 KB an H100 CTA may
+// use.  Two 64 KB park tiles do not fit; one shared tile lets a warpgroup park its whole accumulator before the
+// epilogue, so no accumulator register stays live through it and the existing epilogue code runs unchanged.
 #include <cstdlib>
 
 #include "otb_common.cuh"
@@ -27,13 +33,21 @@ constexpr int kBN = 128;
 constexpr int kBK = 64;
 constexpr int kGemmThreads = 384;   // 2 MMA/epilogue warpgroups + 1 producer warpgroup
 constexpr int kStages = 4;
+constexpr int kGroupM = 32;                         // M-tiles per group of the tile walk
+constexpr int kProducerRegs = 40;                   // setmaxnreg budgets: 40 x 128 + 232 x 256 <= 64 K registers
+constexpr int kMmaRegs = 232;
 constexpr int kABytes = kBM * kBK * 2;              // 16 KB
 constexpr int kBBytes = kBN * kBK * 2;              // 16 KB
 constexpr int kStageBytes = kABytes + kBBytes;
-constexpr int kAccBytes = 64 * kBN * 4;             // one warpgroup's 64 x 128 fp32 tile
+constexpr int kAccBytes = 64 * kBN * 4;             // 64 x 128 fp32: one half of the park tile
+constexpr int kParkBytes = 2 * kAccBytes;           // the 128 x 128 fp32 park tile, 64 KB
 constexpr int kEpiWarpStage = 32 * 128;             // one epilogue warp's store stage: 32 rows x 128 B (64 bf16 columns)
-constexpr int kEpiStageBytes = 8 * kEpiWarpStage;   // 32 KB, sits between the fp32 tiles and the barriers
-constexpr int kGemmSmemBytes = kStages * kStageBytes + 2 * kAccBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int kEpiStageBytes = 8 * kEpiWarpStage;   // 32 KB, sits between the park tile and the barriers
+constexpr int kGemmSmemBytes = kStages * kStageBytes + kParkBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+// named barriers: 1 + wg = the 128 threads of MMA warpgroup wg; kOrderBar + wg = "wg may issue its mainloop";
+// kEpiOrderBar + wg = "wg may fill the park tile"
+constexpr int kOrderBar = 3;
+constexpr int kEpiOrderBar = 5;
 
 struct GemmEpi {
   const float* bias;
@@ -337,11 +351,27 @@ __device__ __forceinline__ void epilogue_dispatch_tma(const GemmEpi& ep, float s
 #undef OTB_EPI_CASE
 }
 
-// Persistent warp-specialised kernel, one CTA per SM.  Warpgroup 2 (one thread) is the TMA producer; warpgroups 0 and 1
-// each own 64 rows of the 128 x 128 tile: 4 wgmma.m64n128k16 per 64-deep k-block, one k-block kept in flight while the
-// next one issues (wait_group 1), its ring slot released as soon as the previous k-block's MMAs retire.  At the end of
-// a tile the warpgroup parks its fragments in its 32 KB fp32 tile and runs the epilogue row by row from there, while
-// the producer already streams the next tile's operands into the ring.
+// Tile t of the launch -> (m0, n0).  Tiles are walked in groups of kGroupM M-tiles, M fastest inside a group, so the
+// operands one wave of CTAs reads stay in L2: at M = 16384, N = 4096, K = 2048 one wave touches ~32 M-tiles x ~4
+// N-tiles, ~18 MB, where an M-fastest walk reads all 64 MB of A per wave.  Launches with tiles_m <= kGroupM keep the
+// plain M-fastest order.  The last group may be narrower (ragged M).
+__device__ __forceinline__ void tile_origin(int t, int tiles_m, int tiles_n, int& m0, int& n0) {
+  const int per_group = kGroupM * tiles_n;
+  const int first_m = (t / per_group) * kGroupM;
+  const int gm = min(kGroupM, tiles_m - first_m);
+  const int r = t % per_group;
+  m0 = (first_m + r % gm) * kBM;
+  n0 = (r / gm) * kBN;
+}
+
+// Persistent warp-specialised ping-pong kernel, one CTA per SM.  Warpgroup 2 (one thread) is the TMA producer and loads
+// the CTA's tiles in order into the ring.  MMA warpgroup wg takes tiles wg, wg + 2, ... of the CTA's sequence and skips
+// the ring slots of the other's tiles.  Per 64-deep k-block it issues 4 k16 steps x 2 wgmma.m64n128k16 (rows 0-63 and
+// 64-127), keeps one k-block in flight while the next one issues (wait_group 1), and releases a ring slot as soon as
+// its MMAs retire.  A named-barrier hand-off orders the mainloops: a warpgroup starts issuing a tile once the other has
+// issued the previous one, so the two alternate on the tensor cores and each one's epilogue runs under the other's
+// mainloop.  Each output element is summed by the same instructions in the same k order as with one warpgroup per
+// 64 rows.
 template <bool A_MN, bool B_MN, bool TS>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -349,8 +379,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* acc_tiles = smem + kStages * kStageBytes;                 // 2 x 32 KB (one per MMA warpgroup)
-  uint8_t* epi_stage = acc_tiles + 2 * kAccBytes;                    // 8 x 4 KB (1024-aligned), TMA-store epilogue only
+  uint8_t* park = smem + kStages * kStageBytes;                      // 64 KB, shared by the MMA warpgroups in turn
+  uint8_t* epi_stage = park + kParkBytes;                            // 8 x 4 KB (1024-aligned), TMA-store epilogue only
   uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + (TS ? kEpiStageBytes : 0));
   uint64_t* full_bar = bars;                        // [kStages]
   uint64_t* empty_bar = bars + kStages;             // [kStages]
@@ -363,13 +393,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   const int tiles_n = (N + kBN - 1) / kBN;
   const int num_tiles = tiles_m * tiles_n;
   const int num_kb = (K + kBK - 1) / kBK;
+  const int cta_tiles = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;   // >= 1: the grid is <= num_tiles
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_b);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 2);   // one arrive per MMA warpgroup
+      mbar_init(&empty_bar[s], 1);   // released by the warpgroup that owns the slot's tile
     }
     fence_mbar_init();
   }
@@ -378,12 +409,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
 
   if (wg == 2) {
     // ===================== TMA producer =====================
+    setmaxnreg_dec<kProducerRegs>();
     if (threadIdx.x == 256) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const int m0 = (t % tiles_m) * kBM;
-        const int n0 = (t / tiles_m) * kBN;
+      for (int i = 0; i < cta_tiles; ++i) {
+        int m0, n0;
+        tile_origin(blockIdx.x + i * gridDim.x, tiles_m, tiles_n, m0, n0);
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * kStageBytes;
@@ -409,58 +441,79 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       }
     }
   } else {
-    // ===================== MMA + epilogue warpgroups: rows [64 wg, 64 wg + 64) of each tile =====================
+    // ===================== MMA + epilogue warpgroups: whole tiles, alternating =====================
+    setmaxnreg_inc<kMmaRegs>();
     constexpr uint32_t a_lbo = A_MN ? kBK * 128 : 16, a_kstep = A_MN ? 2048 : 32;
     constexpr uint32_t b_lbo = B_MN ? kBK * 128 : 16, b_kstep = B_MN ? 2048 : 32;
-    // this warpgroup's 64 rows of A: 8 KB into a K-major tile, the second 64-wide chunk of an MN-major one
+    // rows 64-127 of A: 8 KB into a K-major tile, the second 64-wide chunk of an MN-major one
     constexpr uint32_t a_rows = 64 * 128;
-    uint8_t* acc = acc_tiles + wg * kAccBytes;
     const int q = warp & 1, half = (warp >> 1) & 1;      // epilogue: 32-row quarter of the 64 rows, column half
     float scale = ep.alpha;
     if (ep.scale_ptr != nullptr) {
       const float s = __ldg(ep.scale_ptr);
       scale *= ep.scale_tanh ? tanhf(s) : s;
     }
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const int m0 = (t % tiles_m) * kBM;
-      const int n0 = (t / tiles_m) * kBN;
-      float d[kBN / 2];
+    // it = ring position (k-blocks loaded so far by the producer) of this warpgroup's current tile
+    for (uint32_t i = wg, it = wg * num_kb; i < (uint32_t)cta_tiles; i += 2, it += 2 * num_kb) {
+      int m0, n0;
+      tile_origin(blockIdx.x + i * gridDim.x, tiles_m, tiles_n, m0, n0);
+      float d[2][kBN / 2];
 #pragma unroll
-      for (int i = 0; i < kBN / 2; ++i) d[i] = 0.f;
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < kBN / 2; ++j) d[h][j] = 0.f;
+      if (i > 0) named_bar_sync(kOrderBar + wg, 256);   // the other warpgroup has issued tile i - 1
       int prev_stage = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
+        const int stage = (it + kb) % kStages;
+        mbar_wait(&full_bar[stage], ((it + kb) / kStages) & 1);
         const uint32_t sa = smem_u32(smem + stage * kStageBytes);
         const uint32_t sb = sa + kABytes;
-        const uint64_t da = make_smem_desc(sa + wg * a_rows, a_lbo, 1024);
+        const uint64_t da = make_smem_desc(sa, a_lbo, 1024);
         const uint64_t db = make_smem_desc(sb, b_lbo, 1024);
-        wgmma_keep(d);
+        wgmma_keep(d[0]);
+        wgmma_keep(d[1]);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < kBK / 16; ++k)
-          Wgmma<kBN, A_MN, B_MN>::mma(d, da + ((k * a_kstep) >> 4), db + ((k * b_kstep) >> 4), (kb | k) != 0);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            Wgmma<kBN, A_MN, B_MN>::mma(d[h], da + ((h * a_rows + k * a_kstep) >> 4), db + ((k * b_kstep) >> 4),
+                                        (kb | k) != 0);
         wgmma_commit();
         wgmma_wait<1>();                                 // the previous k-block's MMAs retired: its slot is free
-        wgmma_keep(d);
+        wgmma_keep(d[0]);
+        wgmma_keep(d[1]);
         if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
         prev_stage = stage;
-        if (++stage == kStages) { stage = 0; phase ^= 1; }
       }
+      if (i + 1 < (uint32_t)cta_tiles) named_bar_arrive(kOrderBar + (wg ^ 1), 256);   // hand the tensor cores over
       wgmma_wait<0>();
-      wgmma_keep(d);
+      wgmma_keep(d[0]);
+      wgmma_keep(d[1]);
       if ((threadIdx.x & 127) == 0) mbar_arrive(&empty_bar[prev_stage]);
-      acc_store<kBN>(acc, 0, d);
+      // Epilogue: the whole 128 x 128 fp32 tile is parked in the shared park tile (so no accumulator register stays
+      // live through the epilogue), then the fused epilogue runs on each 64-row half with one thread per (row, column
+      // half).  The two warpgroups' epilogues take turns on the park tile in tile order, like their mainloops.
+      if (i > 0) named_bar_sync(kEpiOrderBar + wg, 256);    // the other warpgroup has finished tile i - 1's epilogue
+      acc_store<kBN>(park, 0, d[0]);
+      acc_store<kBN>(park, 64, d[1]);
       named_bar_sync(1 + wg, 128);
-      if constexpr (TS)
-        epilogue_dispatch_tma<kBN>(ep, scale, acc, m0 + 64 * wg, n0, M, N, q, half, lane, epi_stage + warp * kEpiWarpStage,
-                                   &map_d);
-      else
-        epilogue_tile<kBN>(ep, scale, acc, m0 + 64 * wg, n0, M, N, q, half, lane);
-      named_bar_sync(1 + wg, 128);                      // the fp32 tile is read before the next tile overwrites it
+#pragma unroll 1
+      for (int h = 0; h < 2; ++h) {
+        if constexpr (TS)
+          epilogue_dispatch_tma<kBN>(ep, scale, park + h * kAccBytes, m0 + 64 * h, n0, M, N, q, half, lane,
+                                     epi_stage + warp * kEpiWarpStage, &map_d);
+        else
+          epilogue_tile<kBN>(ep, scale, park + h * kAccBytes, m0 + 64 * h, n0, M, N, q, half, lane);
+      }
+      named_bar_sync(1 + wg, 128);                        // the park tile is read before the other warpgroup refills it
+      if (i + 1 < (uint32_t)cta_tiles) named_bar_arrive(kEpiOrderBar + (wg ^ 1), 256);
+      // the stage must outlive the last bulk store's reads.  Waited for here, inside the loop: the same wait after the
+      // loop makes ptxas allocate the MMA warpgroups' code within the 168-register launch budget instead of the
+      // setmaxnreg one, and the TMA-store epilogue spills.
+      if (TS && i + 2 >= (uint32_t)cta_tiles && lane == 0) tma_store_wait_read<0>();
     }
-    if (TS && lane == 0) tma_store_wait_read<0>();     // the stage must outlive the last bulk store's reads
   }
 }
 
