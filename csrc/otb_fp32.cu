@@ -10,12 +10,6 @@
 
 namespace otb {
 
-__device__ __forceinline__ float warp_sum32(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // pattern 0 (A side): [x0 x0 x1 x1 x0 x2]   pattern 1 (B side): [y0 y1 y0 y1 y2 y0]
 __global__ void split3_concat_kernel(const float* __restrict__ src, long long ld, int rows, int K, int pattern,
                                      bf16* __restrict__ dst) {
@@ -51,10 +45,10 @@ ln_fwd_f32_kernel(const float* __restrict__ x, long long ldx, const float* __res
   const float* xr = x + static_cast<long long>(row) * ldx;
   float s = 0.f;
   for (int c = lane; c < D; c += 32) s += xr[c];
-  const float mean = warp_sum32(s) / D;
+  const float mean = warp_sum(s) / D;
   float ss = 0.f;
   for (int c = lane; c < D; c += 32) { const float d = xr[c] - mean; ss += d * d; }
-  const float rstd = 1.0f / sqrtf(warp_sum32(ss) / D + eps);
+  const float rstd = 1.0f / sqrtf(warp_sum(ss) / D + eps);
   float* yr = y + static_cast<long long>(row) * ldy;
   for (int c = lane; c < D; c += 32) yr[c] = (xr[c] - mean) * rstd * gamma[c] + beta[c];
 }

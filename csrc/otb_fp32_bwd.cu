@@ -10,12 +10,6 @@
 
 namespace otb {
 
-__device__ __forceinline__ float warp_sum_b(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ---- LayerNorm backward: dx (one warp per row) + the row statistics for the parameter pass ----
 __global__ void __launch_bounds__(256)
 ln_bwd_dx_f32_kernel(const float* __restrict__ dy, long long lddy, const float* __restrict__ x, long long ldx,
@@ -30,18 +24,18 @@ ln_bwd_dx_f32_kernel(const float* __restrict__ dy, long long lddy, const float* 
   const float* gr = dy + static_cast<long long>(row) * lddy;
   float s = 0.f;
   for (int c = lane; c < D; c += 32) s += xr[c];
-  const float mean = warp_sum_b(s) / D;
+  const float mean = warp_sum(s) / D;
   float ss = 0.f;
   for (int c = lane; c < D; c += 32) { const float d = xr[c] - mean; ss += d * d; }
-  const float rstd = 1.0f / sqrtf(warp_sum_b(ss) / D + eps);
+  const float rstd = 1.0f / sqrtf(warp_sum(ss) / D + eps);
   float s1 = 0.f, s2 = 0.f;
   for (int c = lane; c < D; c += 32) {
     const float g = gr[c] * gamma[c];
     s1 += g;
     s2 += g * (xr[c] - mean) * rstd;
   }
-  s1 = warp_sum_b(s1) / D;
-  s2 = warp_sum_b(s2) / D;
+  s1 = warp_sum(s1) / D;
+  s2 = warp_sum(s2) / D;
   if (lane == 0) { stats[2 * row] = mean; stats[2 * row + 1] = rstd; }
   if (dx != nullptr) {
     float* o = dx + static_cast<long long>(row) * lddx;

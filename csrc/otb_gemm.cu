@@ -16,13 +16,11 @@
 //                 232).  While one warpgroup runs its mainloop, the other runs the epilogue of its previous tile, so
 //                 the tensor cores do not wait for epilogues.  The epilogue parks the whole accumulator in a swizzled
 //                 fp32 smem tile shared by both warpgroups (their epilogues take turns) and runs the fused
-//                 bias/GELU/gate/residual epilogue with one thread per (row, column half): 16 B stores or a TMA store.
+//                 bias/GELU/gate/residual epilogue with one thread per (row, column half), leaving through TMA stores.
 // Tiles are walked in groups of 32 M-tiles (tile_origin) so one wave's operands stay in L2.
 // Shared memory: 4 x 32 KB ring + 64 KB fp32 park tile + 32 KB TMA-store stage = 224 KB of the 227 KB an H100 CTA may
 // use.  Two 64 KB park tiles do not fit; one shared tile lets a warpgroup park its whole accumulator before the
 // epilogue, so no accumulator register stays live through it and the existing epilogue code runs unchanged.
-#include <cstdlib>
-
 #include "otb_common.cuh"
 #include "otb_host.h"
 
@@ -43,7 +41,8 @@ constexpr int kAccBytes = 64 * kBN * 4;             // 64 x 128 fp32: one half o
 constexpr int kParkBytes = 2 * kAccBytes;           // the 128 x 128 fp32 park tile, 64 KB
 constexpr int kEpiWarpStage = 32 * 128;             // one epilogue warp's store stage: 32 rows x 128 B (64 bf16 columns)
 constexpr int kEpiStageBytes = 8 * kEpiWarpStage;   // 32 KB, sits between the park tile and the barriers
-constexpr int kGemmSmemBytes = kStages * kStageBytes + kParkBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+constexpr int kGemmSmemBytes =
+    kStages * kStageBytes + kParkBytes + kEpiStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 // named barriers: 1 + wg = the 128 threads of MMA warpgroup wg; kOrderBar + wg = "wg may issue its mainloop";
 // kEpiOrderBar + wg = "wg may fill the park tile"
 constexpr int kOrderBar = 3;
@@ -59,137 +58,24 @@ struct GemmEpi {
   long long ld_out, ld_aux_in, ld_aux_out, ld_res;
   int act, scale_tanh, out_fp32, accumulate;
   float alpha;
-  int res_fp32;   // residual is fp32 [M][N] (fp32-grade parity path)
-  int tma_out;    // bf16 output leaves through a swizzled smem stage + TMA store (full 128 B lines, bounds clipped by TMA)
+  int res_fp32;   // residual is fp32 [M][N] (fp32-grade parity path; run-time options only)
   int cls;        // index into kEpiCls when the options match one of the compiled classes, else -1 (run-time options)
 };
 
-
 // One epilogue warp's share of a warpgroup's 64 x BN accumulator tile `acc`: 32-row quarter q, column half `half`.
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
-                                              int N, int q, int half, int lane) {
-  const int row = m0 + q * 32 + lane;
-  const bool row_ok = row < M;
-  const long long lrow = row;
-#pragma unroll 1
-  for (int c = half * (BN / 64); c < (half + 1) * (BN / 64); ++c) {
-    const int colbase = n0 + c * 32;
-    const bool act_chunk = row_ok && colbase < N;
-    // Issue every global read of this 32-column chunk up front (they do not depend on the accumulator):
-    // each thread reads 64 B of its own row, so the loads of a warp are uncoalesced — what matters is
-    // having all of them in flight together instead of one dependent load per 8 columns.
-    uint4 res[4], aux[4];
-    float4 old[8];
-    if (act_chunk) {
-      if (ep.residual != nullptr && !ep.res_fp32) {
-        const uint4* pr = reinterpret_cast<const uint4*>(ep.residual + lrow * ep.ld_res + colbase);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) if (colbase + g * 8 < N) res[g] = __ldg(pr + g);
-      }
-      if (ep.aux_in != nullptr) {
-        const uint4* pa = reinterpret_cast<const uint4*>(ep.aux_in + lrow * ep.ld_aux_in + colbase);
-#pragma unroll
-        for (int g = 0; g < 4; ++g) if (colbase + g * 8 < N) aux[g] = __ldg(pa + g);
-      }
-      if (ep.out_fp32 && ep.accumulate) {
-        const float4* po = reinterpret_cast<const float4*>(reinterpret_cast<float*>(ep.out) + lrow * ep.ld_out + colbase);
-#pragma unroll
-        for (int g = 0; g < 8; ++g) if (colbase + g * 4 < N) old[g] = po[g];
-      }
-    }
-    uint32_t r[32];
-    acc_ld32<BN>(acc, q * 32 + lane, c * 32, r);
-    if (act_chunk) {
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        const int col = colbase + g * 8;
-        if (col >= N) break;
-        float v[8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] = __uint_as_float(r[g * 8 + i]);
-        if (ep.bias != nullptr) {
-          const float4 b0 = __ldg(reinterpret_cast<const float4*>(ep.bias + col));
-          const float4 b1 = __ldg(reinterpret_cast<const float4*>(ep.bias + col + 4));
-          v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
-          v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
-        }
-        if (ep.aux_out != nullptr) {
-          uint4 o;
-          o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-          o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(ep.aux_out + lrow * ep.ld_aux_out + col) = o;
-        }
-        if (ep.aux_in == nullptr) {
-          if (ep.act == 1) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = gelu_fast(v[i]);
-          } else if (ep.act == 2) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) v[i] = quick_gelu(v[i]);
-          } else if (ep.act == 3) {                     // relu^2 (Persimmon "relu2")
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { const float r_ = fmaxf(v[i], 0.f); v[i] = r_ * r_; }
-          }
-        } else {   // backward of the activation whose pre-activation is aux_in: act 3 -> 2 relu(z), otherwise gelu'(z)
-          const float2 a0 = unpack_bf16x2(aux[g].x), a1 = unpack_bf16x2(aux[g].y), a2 = unpack_bf16x2(aux[g].z),
-                       a3 = unpack_bf16x2(aux[g].w);
-          if (ep.act == 3) {
-            v[0] *= 2.f * fmaxf(a0.x, 0.f); v[1] *= 2.f * fmaxf(a0.y, 0.f);
-            v[2] *= 2.f * fmaxf(a1.x, 0.f); v[3] *= 2.f * fmaxf(a1.y, 0.f);
-            v[4] *= 2.f * fmaxf(a2.x, 0.f); v[5] *= 2.f * fmaxf(a2.y, 0.f);
-            v[6] *= 2.f * fmaxf(a3.x, 0.f); v[7] *= 2.f * fmaxf(a3.y, 0.f);
-          } else {
-            v[0] *= gelu_grad_fast(a0.x); v[1] *= gelu_grad_fast(a0.y);
-            v[2] *= gelu_grad_fast(a1.x); v[3] *= gelu_grad_fast(a1.y);
-            v[4] *= gelu_grad_fast(a2.x); v[5] *= gelu_grad_fast(a2.y);
-            v[6] *= gelu_grad_fast(a3.x); v[7] *= gelu_grad_fast(a3.y);
-          }
-        }
-#pragma unroll
-        for (int i = 0; i < 8; ++i) v[i] *= scale;
-        if (ep.residual != nullptr && ep.res_fp32) {
-          const float* pr = reinterpret_cast<const float*>(ep.residual) + lrow * ep.ld_res + col;
-          const float4 r0 = __ldg(reinterpret_cast<const float4*>(pr)), r1 = __ldg(reinterpret_cast<const float4*>(pr + 4));
-          v[0] += r0.x; v[1] += r0.y; v[2] += r0.z; v[3] += r0.w;
-          v[4] += r1.x; v[5] += r1.y; v[6] += r1.z; v[7] += r1.w;
-        } else if (ep.residual != nullptr) {
-          const float2 a0 = unpack_bf16x2(res[g].x), a1 = unpack_bf16x2(res[g].y), a2 = unpack_bf16x2(res[g].z),
-                       a3 = unpack_bf16x2(res[g].w);
-          v[0] += a0.x; v[1] += a0.y; v[2] += a1.x; v[3] += a1.y;
-          v[4] += a2.x; v[5] += a2.y; v[6] += a3.x; v[7] += a3.y;
-        }
-        if (ep.out_fp32) {
-          float* o = reinterpret_cast<float*>(ep.out) + lrow * ep.ld_out + col;
-          float4 o0 = make_float4(0.f, 0.f, 0.f, 0.f), o1 = o0;
-          if (ep.accumulate) { o0 = old[2 * g]; o1 = old[2 * g + 1]; }
-          o0.x += v[0]; o0.y += v[1]; o0.z += v[2]; o0.w += v[3];
-          o1.x += v[4]; o1.y += v[5]; o1.z += v[6]; o1.w += v[7];
-          *reinterpret_cast<float4*>(o) = o0;
-          *reinterpret_cast<float4*>(o + 4) = o1;
-        } else {
-          uint4 o;
-          o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-          o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(reinterpret_cast<bf16*>(ep.out) + lrow * ep.ld_out + col) = o;
-        }
-      }
-    }
-  }
-}
-
-// TMA-store variant of the epilogue.  The direct epilogue above has every thread write 16 B pieces of its own row:
-// 32 different 128 B lines per warp store instruction, partially written sectors on the way to L2, and the
-// accumulate class first READS its old fp32 values the same way.  Here a warp assembles 32 rows x 128 B (64 bf16 or
-// 32 fp32 columns) in a SWIZZLE_128B smem stage — thread = row, the 16 B unit j of row r lands at unit j ^ (r & 7),
-// which is bank-conflict free and exactly the layout the output tensor map expects — and one lane hands the 4 KB box
-// to the TMA engine, which writes whole lines, clips rows >= M / columns >= N, and for `accumulate` performs the
-// fp32 add at L2 (cp.reduce.async.bulk ... add) so the old values never travel to the SM.
+// Stores of 16 B pieces of each thread's own row would touch 32 different 128 B lines per warp store instruction and
+// leave partially written sectors on the way to L2, and an accumulate would first have to READ its old fp32 values
+// the same way.  Instead a warp assembles 32 rows x 128 B (64 bf16 or 32 fp32 columns) in a SWIZZLE_128B smem stage —
+// thread = row, the 16 B unit j of row r lands at unit j ^ (r & 7), which is bank-conflict free and exactly the layout
+// the output tensor map expects — and one lane hands the 4 KB box to the TMA engine, which writes whole lines, clips
+// rows >= M / columns >= N, and for `accumulate` performs the fp32 add at L2 (cp.reduce.async.bulk ... add) so the old
+// values never travel to the SM.
 // The stage is reused once the previous bulk operation has finished READING it (wait_group.read), which overlaps
 // with the accumulator read and the math of the next chunk.  The pre-activation side output (aux_out) keeps direct stores.
 // CLS >= 0: the epilogue options of launch class kEpiCls[CLS] are compile-time constants — the per-group option tests
 // (uniform branches that cut the 32 independent element streams of a chunk into tiny basic blocks) disappear and the
-// chunk becomes one block the scheduler can interleave.  CLS = -1: options read from `ep` at run time (any combination).
+// chunk becomes one block the scheduler can interleave.  CLS = -1: options read from `ep` at run time (any combination,
+// including the fp32 residual).
 struct EpiCls { bool bias, aux_out; int act; bool aux_in, scale, res, out_f32, acc; };
 constexpr int kNumEpiCls = 14;
 constexpr EpiCls kEpiCls[kNumEpiCls] = {
@@ -210,9 +96,9 @@ constexpr EpiCls kEpiCls[kNumEpiCls] = {
 };
 
 template <int BN, int CLS>
-__device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
-                                                  int N, int q, int half, int lane, uint8_t* stage,
-                                                  const CUtensorMap* map_d) {
+__device__ __forceinline__ void epilogue_tile(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
+                                              int N, int q, int half, int lane, uint8_t* stage,
+                                              const CUtensorMap* map_d) {
   constexpr bool kS = CLS >= 0;
   constexpr EpiCls kC = kEpiCls[kS ? CLS : 0];
   const bool f_bias = kS ? kC.bias : (ep.bias != nullptr);
@@ -220,7 +106,8 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
   const int f_act = kS ? kC.act : ep.act;
   const bool f_auxi = kS ? kC.aux_in : (ep.aux_in != nullptr);
   const bool f_scale = kS ? kC.scale : true;
-  const bool f_res = kS ? kC.res : (ep.residual != nullptr);
+  const bool f_res = kS ? kC.res : (ep.residual != nullptr && !ep.res_fp32);   // bf16 residual, loaded up front
+  const bool f_res32 = !kS && ep.residual != nullptr && ep.res_fp32;         // fp32 residual, loaded at its use
   const bool f_f32 = kS ? kC.out_f32 : (ep.out_fp32 != 0);
   const bool f_acc = kS ? kC.acc : (ep.accumulate != 0);
   const int row0 = m0 + q * 32;
@@ -270,12 +157,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
           v[0] += b0.x; v[1] += b0.y; v[2] += b0.z; v[3] += b0.w;
           v[4] += b1.x; v[5] += b1.y; v[6] += b1.z; v[7] += b1.w;
         }
-        if (f_auxo) {
-          uint4 x;
-          x.x = pack_bf16x2(v[0], v[1]); x.y = pack_bf16x2(v[2], v[3]);
-          x.z = pack_bf16x2(v[4], v[5]); x.w = pack_bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(ep.aux_out + lrow * ep.ld_aux_out + col) = x;
-        }
+        if (f_auxo) *reinterpret_cast<uint4*>(ep.aux_out + lrow * ep.ld_aux_out + col) = pack8(v);
         if (!f_auxi) {
           if (f_act == 1) {
 #pragma unroll
@@ -288,18 +170,14 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
             for (int i = 0; i < 8; ++i) { const float r_ = fmaxf(v[i], 0.f); v[i] = r_ * r_; }
           }
         } else {   // backward of the activation whose pre-activation is aux_in: act 3 -> 2 relu(z), otherwise gelu'(z)
-          const float2 a0 = unpack_bf16x2(aux[g].x), a1 = unpack_bf16x2(aux[g].y), a2 = unpack_bf16x2(aux[g].z),
-                       a3 = unpack_bf16x2(aux[g].w);
+          float a[8];
+          unpack8(aux[g], a);
           if (f_act == 3) {
-            v[0] *= 2.f * fmaxf(a0.x, 0.f); v[1] *= 2.f * fmaxf(a0.y, 0.f);
-            v[2] *= 2.f * fmaxf(a1.x, 0.f); v[3] *= 2.f * fmaxf(a1.y, 0.f);
-            v[4] *= 2.f * fmaxf(a2.x, 0.f); v[5] *= 2.f * fmaxf(a2.y, 0.f);
-            v[6] *= 2.f * fmaxf(a3.x, 0.f); v[7] *= 2.f * fmaxf(a3.y, 0.f);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] *= 2.f * fmaxf(a[i], 0.f);
           } else {
-            v[0] *= gelu_grad_fast(a0.x); v[1] *= gelu_grad_fast(a0.y);
-            v[2] *= gelu_grad_fast(a1.x); v[3] *= gelu_grad_fast(a1.y);
-            v[4] *= gelu_grad_fast(a2.x); v[5] *= gelu_grad_fast(a2.y);
-            v[6] *= gelu_grad_fast(a3.x); v[7] *= gelu_grad_fast(a3.y);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) v[i] *= gelu_grad_fast(a[i]);
           }
         }
         if (f_scale) {
@@ -307,10 +185,16 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
           for (int i = 0; i < 8; ++i) v[i] *= scale;
         }
         if (f_res) {
-          const float2 a0 = unpack_bf16x2(res[g].x), a1 = unpack_bf16x2(res[g].y), a2 = unpack_bf16x2(res[g].z),
-                       a3 = unpack_bf16x2(res[g].w);
-          v[0] += a0.x; v[1] += a0.y; v[2] += a1.x; v[3] += a1.y;
-          v[4] += a2.x; v[5] += a2.y; v[6] += a3.x; v[7] += a3.y;
+          float a[8];
+          unpack8(res[g], a);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) v[i] += a[i];
+        }
+        if (f_res32) {
+          const float* pr = reinterpret_cast<const float*>(ep.residual) + lrow * ep.ld_res + col;
+          const float4 r0 = __ldg(reinterpret_cast<const float4*>(pr)), r1 = __ldg(reinterpret_cast<const float4*>(pr + 4));
+          v[0] += r0.x; v[1] += r0.y; v[2] += r0.z; v[3] += r0.w;
+          v[4] += r1.x; v[5] += r1.y; v[6] += r1.z; v[7] += r1.w;
         }
       }
       // rows >= M and columns >= N hold don't-care values: the TMA engine clips them
@@ -318,10 +202,7 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
         *reinterpret_cast<float4*>(my_row + (((2 * g) ^ xr) << 4)) = make_float4(v[0], v[1], v[2], v[3]);
         *reinterpret_cast<float4*>(my_row + (((2 * g + 1) ^ xr) << 4)) = make_float4(v[4], v[5], v[6], v[7]);
       } else {
-        uint4 o;
-        o.x = pack_bf16x2(v[0], v[1]); o.y = pack_bf16x2(v[2], v[3]);
-        o.z = pack_bf16x2(v[4], v[5]); o.w = pack_bf16x2(v[6], v[7]);
-        *reinterpret_cast<uint4*>(my_row + ((((c & 1) * 4 + g) ^ xr) << 4)) = o;
+        *reinterpret_cast<uint4*>(my_row + ((((c & 1) * 4 + g) ^ xr) << 4)) = pack8(v);
       }
     }
     if (last_of_box) {
@@ -339,14 +220,14 @@ __device__ __forceinline__ void epilogue_tile_tma(const GemmEpi& ep, float scale
 
 // per-tile dispatch on the launch's epilogue class (host: epi_class_of)
 template <int BN>
-__device__ __forceinline__ void epilogue_dispatch_tma(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0,
-                                                      int M, int N, int q, int half, int lane, uint8_t* stage,
-                                                      const CUtensorMap* map_d) {
-#define OTB_EPI_CASE(C_) case C_: epilogue_tile_tma<BN, C_>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
+__device__ __forceinline__ void epilogue_dispatch(const GemmEpi& ep, float scale, uint8_t* acc, int m0, int n0, int M,
+                                                  int N, int q, int half, int lane, uint8_t* stage,
+                                                  const CUtensorMap* map_d) {
+#define OTB_EPI_CASE(C_) case C_: epilogue_tile<BN, C_>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
   switch (ep.cls) {
     OTB_EPI_CASE(0) OTB_EPI_CASE(1) OTB_EPI_CASE(2) OTB_EPI_CASE(3) OTB_EPI_CASE(4) OTB_EPI_CASE(5) OTB_EPI_CASE(6)
     OTB_EPI_CASE(7) OTB_EPI_CASE(8) OTB_EPI_CASE(9) OTB_EPI_CASE(10) OTB_EPI_CASE(11) OTB_EPI_CASE(12) OTB_EPI_CASE(13)
-    default: epilogue_tile_tma<BN, -1>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
+    default: epilogue_tile<BN, -1>(ep, scale, acc, m0, n0, M, N, q, half, lane, stage, map_d); break;
   }
 #undef OTB_EPI_CASE
 }
@@ -372,7 +253,7 @@ __device__ __forceinline__ void tile_origin(int t, int tiles_m, int tiles_n, int
 // issued the previous one, so the two alternate on the tensor cores and each one's epilogue runs under the other's
 // mainloop.  Each output element is summed by the same instructions in the same k order as with one warpgroup per
 // 64 rows.
-template <bool A_MN, bool B_MN, bool TS>
+template <bool A_MN, bool B_MN>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
                  const __grid_constant__ CUtensorMap map_d, int M, int N, int K, GemmEpi ep) {
@@ -380,8 +261,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* park = smem + kStages * kStageBytes;                      // 64 KB, shared by the MMA warpgroups in turn
-  uint8_t* epi_stage = park + kParkBytes;                            // 8 x 4 KB (1024-aligned), TMA-store epilogue only
-  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + (TS ? kEpiStageBytes : 0));
+  uint8_t* epi_stage = park + kParkBytes;                            // 8 x 4 KB (1024-aligned), one per epilogue warp
+  uint64_t* bars = reinterpret_cast<uint64_t*>(epi_stage + kEpiStageBytes);
   uint64_t* full_bar = bars;                        // [kStages]
   uint64_t* empty_bar = bars + kStages;             // [kStages]
 
@@ -500,27 +381,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constan
       acc_store<kBN>(park, 64, d[1]);
       named_bar_sync(1 + wg, 128);
 #pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        if constexpr (TS)
-          epilogue_dispatch_tma<kBN>(ep, scale, park + h * kAccBytes, m0 + 64 * h, n0, M, N, q, half, lane,
-                                     epi_stage + warp * kEpiWarpStage, &map_d);
-        else
-          epilogue_tile<kBN>(ep, scale, park + h * kAccBytes, m0 + 64 * h, n0, M, N, q, half, lane);
-      }
+      for (int h = 0; h < 2; ++h)
+        epilogue_dispatch<kBN>(ep, scale, park + h * kAccBytes, m0 + 64 * h, n0, M, N, q, half, lane,
+                               epi_stage + warp * kEpiWarpStage, &map_d);
       named_bar_sync(1 + wg, 128);                        // the park tile is read before the other warpgroup refills it
       if (i + 1 < (uint32_t)cta_tiles) named_bar_arrive(kEpiOrderBar + (wg ^ 1), 256);
       // the stage must outlive the last bulk store's reads.  Waited for here, inside the loop: the same wait after the
       // loop makes ptxas allocate the MMA warpgroups' code within the 168-register launch budget instead of the
-      // setmaxnreg one, and the TMA-store epilogue spills.
-      if (TS && i + 2 >= (uint32_t)cta_tiles && lane == 0) tma_store_wait_read<0>();
+      // setmaxnreg one, and the epilogue spills.
+      if (i + 2 >= (uint32_t)cta_tiles && lane == 0) tma_store_wait_read<0>();
     }
   }
 }
 
-template <bool A_MN, bool B_MN, bool TS>
+template <bool A_MN, bool B_MN>
 static int launch_gemm(const void* A, long long lda, const void* B, long long ldb, int M, int N, int K,
                        const GemmEpi& ep, cudaStream_t stream) {
-  CUtensorMap ma, mb;
+  CUtensorMap ma, mb, md;
   int rc;
   if (!A_MN) rc = make_tmap_bf16_2d(&ma, A, M, K, lda, kBM, 64);   // [M][K], box 128 rows x 64 k
   else       rc = make_tmap_bf16_2d(&ma, A, K, M, lda, kBK, 64);   // [K][M], box 64 k-rows x 64 m
@@ -528,15 +405,11 @@ static int launch_gemm(const void* A, long long lda, const void* B, long long ld
   if (!B_MN) rc = make_tmap_bf16_2d(&mb, B, N, K, ldb, kBN, 64);
   else       rc = make_tmap_bf16_2d(&mb, B, K, N, ldb, kBK, 64);
   if (rc) return rc;
-  CUtensorMap md = ma;                                               // placeholder when the direct epilogue is used
-  if (TS) {                                                          // [M][N] output, box 32 rows x 128 B
-    rc = ep.out_fp32 ? make_tmap_f32_2d(&md, ep.out, M, N, ep.ld_out, 32, 32)
-                     : make_tmap_bf16_2d(&md, ep.out, M, N, ep.ld_out, 32, 64);
-    if (rc) return rc;
-  }
-  auto kern = gemm_bf16_kernel<A_MN, B_MN, TS>;
-  constexpr int smem_bytes = kGemmSmemBytes + (TS ? kEpiStageBytes : 0);
-  OTB_CHECK_CUDA(ensure_dyn_smem(kern, smem_bytes));   // per (instantiation, device)
+  rc = ep.out_fp32 ? make_tmap_f32_2d(&md, ep.out, M, N, ep.ld_out, 32, 32)    // [M][N] output, box 32 rows x 128 B
+                   : make_tmap_bf16_2d(&md, ep.out, M, N, ep.ld_out, 32, 64);
+  if (rc) return rc;
+  auto kern = gemm_bf16_kernel<A_MN, B_MN>;
+  OTB_CHECK_CUDA(ensure_dyn_smem(kern, kGemmSmemBytes));   // per (instantiation, device)
   const int tiles = ((M + kBM - 1) / kBM) * ((N + kBN - 1) / kBN);
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
@@ -550,7 +423,7 @@ static int launch_gemm(const void* A, long long lda, const void* B, long long ld
   cfg.attrs = attr;
   cfg.numAttrs = nattr;
   cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = smem_bytes;
+  cfg.dynamicSmemBytes = kGemmSmemBytes;
   cfg.stream = stream;
   OTB_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, ma, mb, md, M, N, K, ep));
   count_launch();
@@ -563,6 +436,8 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
                              int M, int N, int K, const otb_gemm_epilogue* e, void* stream) {
   using namespace otb;
   OTB_CHECK_ARG(A && B && e && e->out, "otb_gemm_bf16: null pointer");
+  // the output tensor map of the TMA-store epilogue needs a 16-byte aligned base
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->out) & 15) == 0, "otb_gemm_bf16: out must be 16-byte aligned");
   OTB_CHECK_ARG(M > 0 && N > 0 && K > 0, "otb_gemm_bf16: bad shape %d %d %d", M, N, K);
   OTB_CHECK_ARG(N % 8 == 0, "otb_gemm_bf16: N=%d must be a multiple of 8", N);
   OTB_CHECK_ARG(e->ld_out % 8 == 0 && e->ld_out >= N, "otb_gemm_bf16: bad ld_out");
@@ -589,13 +464,8 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
   ep.alpha = e->alpha;
   ep.res_fp32 = e->res_fp32;
   OTB_CHECK_ARG(!e->res_fp32 || e->out_fp32, "otb_gemm_bf16: fp32 residual requires fp32 output");
-  // Outputs leave through the smem-staged TMA-store / reduce-add epilogue (full 128 B lines, fp32 accumulate performed
-  // at L2).  OTB_GEMM_EPI_TMA=0 selects direct stores.
-  static const bool epi_tma = [] { const char* v = getenv("OTB_GEMM_EPI_TMA"); return !(v && v[0] == '0'); }();
-  ep.tma_out = (epi_tma && !e->res_fp32 && (reinterpret_cast<uintptr_t>(e->out) & 15) == 0 &&
-                (!e->out_fp32 || e->ld_out % 4 == 0)) ? 1 : 0;
   ep.cls = -1;
-  if (ep.tma_out && e->res_fp32 == 0) {
+  if (e->res_fp32 == 0) {                                   // the fp32 residual takes the run-time options
     const bool scaled = (e->scale_ptr != nullptr) || e->alpha != 1.0f;
     for (int c = 0; c < kNumEpiCls; ++c) {
       const EpiCls& k = kEpiCls[c];
@@ -607,20 +477,14 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
       }
     }
   }
-  static const bool cls_off = [] { const char* v = getenv("OTB_GEMM_EPI_CLS"); return v && v[0] == '0'; }();
-  if (cls_off) ep.cls = -1;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
 
   const int sel = (a_mn_major ? 2 : 0) | (b_mn_major ? 1 : 0);
-#define OTB_GEMM_CASE(A_, B_)                                                    \
-  return ep.tma_out ? launch_gemm<A_, B_, true>(A, lda, B, ldb, M, N, K, ep, st) \
-                    : launch_gemm<A_, B_, false>(A, lda, B, ldb, M, N, K, ep, st)
   switch (sel) {
-    case 0: OTB_GEMM_CASE(false, false);
-    case 1: OTB_GEMM_CASE(false, true);
-    case 3: OTB_GEMM_CASE(true, true);
+    case 0: return launch_gemm<false, false>(A, lda, B, ldb, M, N, K, ep, st);
+    case 1: return launch_gemm<false, true>(A, lda, B, ldb, M, N, K, ep, st);
+    case 3: return launch_gemm<true, true>(A, lda, B, ldb, M, N, K, ep, st);
     default: break;
   }
-#undef OTB_GEMM_CASE
   return set_error(OTB_ERR_UNSUPPORTED, "otb_gemm_bf16: layout (A MN-major, B K-major) not instantiated");
 }

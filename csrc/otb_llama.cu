@@ -10,21 +10,6 @@
 
 namespace otb {
 
-__device__ __forceinline__ float warp_sum_f(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ void unpack8f(uint4 u, float (&f)[8]) {
-  const float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-__device__ __forceinline__ uint4 pack8f(const float (&f)[8]) {
-  uint4 u;
-  u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]); u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
-  return u;
-}
-
 // one warp per row; D % 8 == 0
 __global__ void __launch_bounds__(256)
 rmsnorm_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __restrict__ w, bf16* __restrict__ y,
@@ -39,21 +24,21 @@ rmsnorm_fwd_kernel(const bf16* __restrict__ x, long long ldx, const float* __res
   float ss = 0.f;
   for (int v = lane; v < nvec; v += 32) {
     float f[8];
-    unpack8f(__ldg(px + v), f);
+    unpack8(__ldg(px + v), f);
 #pragma unroll
     for (int i = 0; i < 8; ++i) ss += f[i] * f[i];
   }
-  const float rstd = rsqrtf(warp_sum_f(ss) / D + eps);
+  const float rstd = rsqrtf(warp_sum(ss) / D + eps);
   if (lane == 0 && rstd_out != nullptr) rstd_out[row] = rstd;
   uint4* py = reinterpret_cast<uint4*>(y + static_cast<long long>(row) * ldy);
   for (int v = lane; v < nvec; v += 32) {
     float f[8];
-    unpack8f(__ldg(px + v), f);
+    unpack8(__ldg(px + v), f);
     const float4 w0 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v), w1 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v + 1);
     const float ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
     for (int i = 0; i < 8; ++i) f[i] = f[i] * rstd * ww[i];
-    py[v] = pack8f(f);
+    py[v] = pack8(f);
   }
 }
 
@@ -74,21 +59,21 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __re
   float s = 0.f;
   for (int v = lane; v < nvec; v += 32) {
     float fx[8], fd[8];
-    unpack8f(__ldg(px + v), fx);
-    unpack8f(__ldg(pd + v), fd);
+    unpack8(__ldg(px + v), fx);
+    unpack8(__ldg(pd + v), fd);
     const float4 w0 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v), w1 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v + 1);
     const float ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
     for (int i = 0; i < 8; ++i) s += fd[i] * ww[i] * fx[i] * rstd;
   }
-  const float m = warp_sum_f(s) / D;
+  const float m = warp_sum(s) / D;
   uint4* po = reinterpret_cast<uint4*>(dx + static_cast<long long>(row) * lddx);
   const uint4* pa = add ? reinterpret_cast<const uint4*>(add + static_cast<long long>(row) * ldadd) : nullptr;
   for (int v = lane; v < nvec; v += 32) {
     float fx[8], fd[8], fa[8], o[8];
-    unpack8f(__ldg(px + v), fx);
-    unpack8f(__ldg(pd + v), fd);
-    if (pa) unpack8f(__ldg(pa + v), fa);
+    unpack8(__ldg(px + v), fx);
+    unpack8(__ldg(pd + v), fd);
+    if (pa) unpack8(__ldg(pa + v), fa);
     const float4 w0 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v), w1 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v + 1);
     const float ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
@@ -96,7 +81,7 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __re
       o[i] = rstd * (fd[i] * ww[i] - fx[i] * rstd * m);
       if (pa) o[i] += fa[i];
     }
-    po[v] = pack8f(o);
+    po[v] = pack8(o);
   }
 }
 
@@ -143,11 +128,11 @@ swiglu_fwd_kernel(const bf16* __restrict__ g, long long ldg, const bf16* __restr
     const long long row = idx / nvec;
     const int v = static_cast<int>(idx % nvec);
     float fg[8], fu[8], o[8];
-    unpack8f(__ldg(reinterpret_cast<const uint4*>(g + row * ldg) + v), fg);
-    unpack8f(__ldg(reinterpret_cast<const uint4*>(u + row * ldu) + v), fu);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(g + row * ldg) + v), fg);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(u + row * ldu) + v), fu);
 #pragma unroll
     for (int i = 0; i < 8; ++i) o[i] = fg[i] * sigmoidf_(fg[i]) * fu[i];
-    reinterpret_cast<uint4*>(h + row * ldh)[v] = pack8f(o);
+    reinterpret_cast<uint4*>(h + row * ldh)[v] = pack8(o);
   }
 }
 
@@ -165,17 +150,17 @@ swiglu_bwd_kernel(const bf16* __restrict__ dh, long long lddh, const bf16* __res
     const long long row = idx / nvec;
     const int v = static_cast<int>(idx % nvec);
     float fd[8], fg[8], fu[8], og[8], ou[8];
-    unpack8f(__ldg(reinterpret_cast<const uint4*>(dh + row * lddh) + v), fd);
-    unpack8f(__ldg(reinterpret_cast<const uint4*>(g + row * ldg) + v), fg);
-    unpack8f(__ldg(reinterpret_cast<const uint4*>(u + row * ldu) + v), fu);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(dh + row * lddh) + v), fd);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(g + row * ldg) + v), fg);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(u + row * ldu) + v), fu);
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
       const float sg = sigmoidf_(fg[i]);
       og[i] = fd[i] * fu[i] * (sg + fg[i] * sg * (1.0f - sg));
       ou[i] = fd[i] * fg[i] * sg;
     }
-    reinterpret_cast<uint4*>(dg + row * lddg)[v] = pack8f(og);
-    reinterpret_cast<uint4*>(du + row * lddu)[v] = pack8f(ou);
+    reinterpret_cast<uint4*>(dg + row * lddg)[v] = pack8(og);
+    reinterpret_cast<uint4*>(du + row * lddu)[v] = pack8(ou);
   }
 }
 

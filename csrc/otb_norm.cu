@@ -1,28 +1,10 @@
 // otter_b200 — HBM-bound passes of the hot path: LayerNorm fwd/bwd, mask index construction,
 // casts, broadcast / grouped reductions, tanh-gate gradient, CLIP embedding assembly, Fuyu scatter.
 // All are plain coalesced, 16-byte-vectorised CUDA kernels (no tensor cores: byte/element work).
-#include <cstdlib>
-
 #include "otb_common.cuh"
 #include "otb_host.h"
 
 namespace otb {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-__device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
-  float2 a = unpack_bf16x2(u.x), b = unpack_bf16x2(u.y), c = unpack_bf16x2(u.z), d = unpack_bf16x2(u.w);
-  f[0] = a.x; f[1] = a.y; f[2] = b.x; f[3] = b.y; f[4] = c.x; f[5] = c.y; f[6] = d.x; f[7] = d.y;
-}
-__device__ __forceinline__ uint4 pack8(const float (&f)[8]) {
-  uint4 u;
-  u.x = pack_bf16x2(f[0], f[1]); u.y = pack_bf16x2(f[2], f[3]);
-  u.z = pack_bf16x2(f[4], f[5]); u.w = pack_bf16x2(f[6], f[7]);
-  return u;
-}
 
 // ------------------------------------------------------------------------------------------------
 // LayerNorm forward: one warp per row, 3 sweeps over the row (2nd/3rd hit L1), fp32 statistics.
@@ -158,7 +140,7 @@ ln_bwd_param_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __r
     if (gc < D) ws[(static_cast<long long>(which) * chunks + chunk) * D + gc] = acc;
   }
 }
-// One-pass LayerNorm backward (default; OTB_LN_FUSED=0 selects the three-kernel path): dx AND the gamma/beta column partials from a single read of
+// One-pass LayerNorm backward (D <= 4096): dx AND the gamma/beta column partials from a single read of
 // x / dy.  A CTA walks its rows in batches of kLnR; thread t owns the 16 B column vectors t, t+256, ... (VPT of them) of
 // every row, so the parameter partials stay in its registers across all rows of the CTA (deterministic: fixed order,
 // no atomics) and the two row statistics of a batch take one block reduction (double-buffered smem, one barrier).
@@ -707,17 +689,13 @@ extern "C" int otb_layernorm_fwd(const void* x, int64_t ldx, const float* gamma,
   return OTB_OK;
 }
 
-static bool ln_fused_enabled() {
-  static const bool on = [] { const char* e = getenv("OTB_LN_FUSED"); return !(e && e[0] == '0'); }();   // default on
-  return on;
-}
 static int ln_fused_grid(int rows) {
   const int nbatch = (rows + otb::kLnR - 1) / otb::kLnR;
   return nbatch < otb::sm_count() ? nbatch : otb::sm_count();
 }
 
 extern "C" int otb_ln_chunks(int rows, int D) {
-  if (ln_fused_enabled() && D <= 4096) {        // workspace must hold one partial row per CTA of the one-pass kernel
+  if (D <= 4096) {        // workspace must hold one partial row per CTA of the one-pass kernel
     const int g = ln_fused_grid(rows);
     int colblocks0 = (D + 63) / 64, chunks0 = (4 * 132 + colblocks0 - 1) / colblocks0;   // 4 x the H100's SMs
     return g > chunks0 ? g : chunks0;
@@ -735,9 +713,11 @@ extern "C" int otb_layernorm_bwd(const void* dy, int64_t lddy, const void* x, in
                                  int D, void* stream) {
   OTB_CHECK_ARG(dy && x && mean && rstd && gamma && rows > 0 && D > 0, "otb_layernorm_bwd: bad argument");
   OTB_CHECK_ARG(D % 8 == 0 && lddy % 8 == 0 && ldx % 8 == 0, "otb_layernorm_bwd: D/ld must be multiples of 8");
-  // dx == nullptr (perceiver norm_media: the frozen CLIP features need no input gradient) takes the one-pass kernel too:
-  // it then only produces the gamma / beta partials, one launch instead of the three-kernel fallback
-  if (ln_fused_enabled() && D <= 4096 && (dgamma != nullptr || dbeta != nullptr)) {
+  // Parameter gradients take the one-pass kernel, which holds at most two 16 B vectors of a row per thread (D <= 4096);
+  // wider rows take ln_bwd_dx_kernel + the param / finalize kernels below.  dx == nullptr (perceiver norm_media: the
+  // frozen CLIP features need no input gradient) takes the one-pass kernel too: it then only produces the gamma / beta
+  // partials.  Only dx wanted (the frozen MPT / Persimmon layers): ln_bwd_dx_kernel alone.
+  if (D <= 4096 && (dgamma != nullptr || dbeta != nullptr)) {
     OTB_CHECK_ARG((dx == nullptr || lddx % 8 == 0) && (add == nullptr || ldadd % 8 == 0), "otb_layernorm_bwd: bad ld");
     OTB_CHECK_ARG(ws != nullptr, "otb_layernorm_bwd: workspace required for parameter gradients");
     const int grid = ln_fused_grid(rows);

@@ -18,12 +18,6 @@ namespace otb {
 constexpr int kQkBlock = 256;            // 8 warps
 constexpr int kQkMaxBlocks = 592;        // 4 per SM: partial [blocks][4][64] rows of the parameter-gradient reduction
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // cos / sin of the rotary angle for rotary dim index i (0 <= i < rot): angle = pos * theta^(-2 (i mod rot/2) / rot)
 __device__ __forceinline__ void rope_cs(int pos, int i, int rot, float log2_theta, float& c, float& s) {
   const int half = rot >> 1;

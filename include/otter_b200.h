@@ -50,8 +50,8 @@ int otb_abi_sizeof(int which);
  *   a_mn_major = 1 : A is stored [K][M] row-major (lda >= M)         (dY^T for wgrad, no transpose copy)
  *   b_mn_major = 0 : B is stored [N][K] row-major (ldb >= K)         (nn.Linear weight for forward)
  *   b_mn_major = 1 : B is stored [K][N] row-major (ldb >= N)         (weight for dgrad, X for wgrad)
- * Requirements: lda, ldb, ld_out, ld_aux, ld_res multiples of 8; pointers 16-byte aligned;
- *   N multiple of 8; for an MN-major operand its MN extent must be a multiple of 8.
+ * Requirements: lda, ldb, ld_out, ld_aux, ld_res multiples of 8; pointers 16-byte aligned (a misaligned `out`
+ *   returns OTB_ERR_INVALID); N multiple of 8; for an MN-major operand its MN extent must be a multiple of 8.
  *
  * Epilogue (all optional, applied in this order on the fp32 accumulator v):
  *   v += bias[n]                                   (fp32 [N])
@@ -63,7 +63,7 @@ int otb_abi_sizeof(int which);
  *                                                   any other value -> gelu'(z))
  *   v *= alpha * (scale_ptr ? (scale_tanh ? tanh(*scale_ptr) : *scale_ptr) : 1)
  *                                                  (tanh gate, modeling_otter.py:387-388,393)
- *   v += residual[m,n]                             (bf16)
+ *   v += residual[m,n]                             (bf16, or fp32 when res_fp32)
  *   out[m,n] = (accumulate ? out[m,n] : 0) + v     (bf16, or fp32 when out_fp32; accumulate needs fp32)
  * ------------------------------------------------------------------------------------------- */
 typedef struct otb_gemm_epilogue {
@@ -79,7 +79,8 @@ typedef struct otb_gemm_epilogue {
   int32_t out_fp32;
   int32_t accumulate;
   float alpha;
-  int32_t res_fp32; /* residual is fp32 [M][N] instead of bf16 (fp32-grade parity path; needs out_fp32) */
+  int32_t res_fp32; /* residual is fp32 [M][N] instead of bf16 (fp32-grade parity path; needs out_fp32).  Runs the
+                       epilogue with run-time options rather than one specialised for a launch class. */
 } otb_gemm_epilogue;
 
 int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const void* B, int b_mn_major, int64_t ldb, int M,

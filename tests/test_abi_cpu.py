@@ -41,6 +41,10 @@ def test_invalid_arguments_return_error_codes():
     e = _lib.GemmEpilogue()
     rc = lib.otb_gemm_bf16(None, 0, 0, None, 0, 0, 0, 0, 0, C.byref(e), None)
     assert rc == 1 and b"otb_gemm_bf16" in lib.otb_last_error()
+    # valid shapes, 16-byte aligned A / B, an output 2 bytes past a 16-byte boundary: rejected before any launch
+    e.out, e.ld_out = 0x10002, 128
+    rc = lib.otb_gemm_bf16(0x10000, 0, 128, 0x20000, 0, 128, 128, 128, 128, C.byref(e), None)
+    assert rc == 1 and b"aligned" in lib.otb_last_error()
     assert lib.otb_text_time(None, 0, 0, 1, None, None) == 1
     assert lib.otb_layernorm_fwd(None, 0, None, None, None, 0, None, None, 0, 0, 1e-5, None) == 1
     d = _lib.AttnDesc()

@@ -1,4 +1,4 @@
-"""CPU model of the TMA-store epilogue's addressing (csrc/otb_gemm.cu epilogue_tile_tma): every lane writes its 16 B
+"""CPU model of the TMA-store epilogue's addressing (csrc/otb_gemm.cu epilogue_tile): every lane writes its 16 B
 units into the warp's SWIZZLE_128B stage exactly as the kernel does; a model of the TMA engine (de-swizzle by
 unit ^ (row & 7), clip the 32-row x 128-byte box against the tensor) stores it.  The result must equal the plain
 tile for bf16 and fp32 outputs, full and ragged M / N, BN = 128 and 256."""

@@ -84,8 +84,10 @@ def test_grouped_walk_ragged_last_group(layout):
         assert_close(F.linear_wgrad(dy, x), dy.float().t() @ x.float(), F32_RTOL, F32_ATOL, layout)
 
 
-# every compiled epilogue class (kEpiCls in otb_gemm.cu) and the direct-store fp32-residual path, at 8 x 64 = 512 tiles
-@pytest.mark.parametrize("cls", list(range(14)) + ["res_fp32"])
+# every compiled epilogue class (kEpiCls in otb_gemm.cu), and the run-time epilogue options with each combination the
+# hot path uses outside those classes: fp32 residual (fp32-grade forward), bias + relu^2 + pre-activation (Persimmon
+# up-projection), relu^2'(aux) (Persimmon dgrad), bias + GELU into fp32 (fp32-grade forward); at 8 x 64 = 512 tiles
+@pytest.mark.parametrize("cls", list(range(14)) + ["res_fp32", "relu2_aux_out", "relu2_grad", "gelu_f32"])
 def test_epilogue_classes(cls):
     from otter_b200 import functional as F
     M, N, K = 1024, 8192, 128
@@ -133,11 +135,19 @@ def test_epilogue_classes(cls):
         epi = dict(scale_ptr=gate, scale_tanh=True) if cls == 13 else {}
         got = F._gemm_raw(x, 0, x.stride(0), w, 0, w.stride(0), M, N, K, old.clone(), accumulate=True, **epi)
         ref, tol = old + zr * (g if cls == 13 else 1.0), f32
-    else:                                          # fp32 residual: the direct-store epilogue
+    elif cls == "res_fp32":
         res32 = torch.randn(M, N, device=dev(), generator=torch.Generator(device=dev()).manual_seed(11))
         out = torch.empty(M, N, device=dev())
         got = F._gemm_raw(x, 0, x.stride(0), w, 0, w.stride(0), M, N, K, out, residual=res32, res_fp32=True)
         ref, tol = zr + res32, f32
+    elif cls == "relu2_aux_out":
+        got, ref, tol = F.linear_fwd(x, w, bias=bias, act=3, aux_out=z), torch.relu(zr + bias) ** 2, bf
+        assert_close(z, zr + bias, *bf, "aux_out")
+    elif cls == "relu2_grad":
+        got, ref, tol = F.linear_fwd(x, w, aux_in=aux, act=3), zr * 2 * torch.relu(aux.float()), bf
+    else:
+        got = F.linear_fwd(x, w, bias=bias, act=1, out_dtype=torch.float32)
+        ref, tol = torch.nn.functional.gelu(zr + bias), f32
     assert_close(got, ref, *tol, f"class {cls}")
 
 
