@@ -1,6 +1,6 @@
 """GPU: BASELINE.json full-size shapes, checked through size-independent properties and (where the CPU oracle
 finishes in seconds) directly against oracle/restatement.py.  c2: D=4096, L=256, batch 8; c3: video F=8
-(2048+64 keys -> streaming attention kernel); c5: Fuyu patch-linear 1225 x 2700 -> 4096 + scatter."""
+(2048+64 keys = 17 key tiles of the attention kernels); c5: Fuyu patch-linear 1225 x 2700 -> 4096 + scatter."""
 import pytest
 import torch
 
@@ -47,7 +47,8 @@ def test_c2_gated_block_properties():
 
 
 def test_c3_video_perceiver_streaming_attention():
-    """F=8 frames -> 2048 media keys + 64 latents = 17 key tiles: the streaming two-sweep kernel, fwd + bwd."""
+    """F=8 frames -> 2048 media keys + 64 latents = 17 key tiles streamed through the double-buffered TMA ring: the
+    two-sweep forward and the dQ workspace of the backward, fwd + bwd."""
     from otter_b200.modeling_otter import OtterPerceiverResampler
     torch.manual_seed(1)
     rs = OtterPerceiverResampler(dim=1024, depth=2, max_num_frames=16).to(DEV)

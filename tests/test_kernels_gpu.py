@@ -103,95 +103,6 @@ def test_text_time_bit_exact():
             assert got.dtype == np.int32 and np.array_equal(got.astype(np.int64), ref), (L, ap)
 
 
-def _attn_ref(q, k, v, scale, tt=None, n=64, T=1):
-    """fp32 reference of the attention core with the reference's mask semantics. q [P,H,Sq,64] etc."""
-    sim = (q * scale) @ k.transpose(-1, -2)
-    if tt is not None:
-        media_time = torch.arange(T, device=q.device).repeat_interleave(n) + 1
-        keep = tt[:, None, :, None] == media_time[None, None, None, :]
-        sim = sim.masked_fill(~keep, -torch.finfo(sim.dtype).max)
-    sim = sim - sim.amax(dim=-1, keepdim=True).detach()
-    attn = sim.softmax(dim=-1)
-    if tt is not None:
-        attn = attn.masked_fill((tt == 0)[:, None, :, None], 0.0)
-    return attn @ v
-
-
-def _heads(t, P, S, H):
-    return t.float().reshape(P, S, H, 64).permute(0, 2, 1, 3)
-
-
-@pytest.mark.parametrize("P,H,Sq,Sk1,Sk2", [(2, 8, 64, 256, 64), (1, 2, 64, 96, 64), (3, 4, 257, 257, 0),
-                                             (2, 2, 64, 2048, 64), (2, 8, 300, 64, 0),
-                                             # >= 119 (problem, head) pairs: one CTA walks ALL query tiles with K/V resident
-                                             (8, 16, 257, 257, 0), (16, 8, 300, 64, 0), (15, 8, 700, 130, 64)])
-def test_attention_fwd_bwd_unmasked(P, H, Sq, Sk1, Sk2):
-    from otter_b200 import functional as F
-    inner = H * 64
-    q = rnd(P * Sq, inner, seed=1)
-    kv1 = rnd(P * Sk1, 2 * inner, seed=2)
-    kv2 = rnd(P * Sk2, 2 * inner, seed=3) if Sk2 else None
-    spec = F.AttnSpec(q, 0, kv1, 0, inner, P, H, Sq, Sk1, 0.125, kv2=kv2, k2_col0=0, v2_col0=inner, Sk2=Sk2)
-    out, lse = F.attn_fwd(spec)
-    qr = q.float().requires_grad_(True)
-    k1r = kv1.float().requires_grad_(True)
-    k2r = kv2.float().requires_grad_(True) if Sk2 else None
-    kk = _heads(k1r[:, :inner], P, Sk1, H)
-    vv = _heads(k1r[:, inner:], P, Sk1, H)
-    if Sk2:
-        kk = torch.cat([kk, _heads(k2r[:, :inner], P, Sk2, H)], dim=2)
-        vv = torch.cat([vv, _heads(k2r[:, inner:], P, Sk2, H)], dim=2)
-    ref = _attn_ref(_heads(qr, P, Sq, H), kk, vv, 0.125).permute(0, 2, 1, 3).reshape(P * Sq, inner)
-    assert_close(out, ref, 2e-2, 2e-2, "attn fwd")
-    dout = rnd(P * Sq, inner, seed=5)
-    ref.backward(dout.float())
-    dq = torch.zeros_like(q)
-    dkv1 = torch.zeros_like(kv1)
-    dkv2 = torch.zeros_like(kv2) if Sk2 else None
-    F.attn_bwd(spec, out, 0, lse, dout, 0, dq, 0, dkv1, 0, inner, dkv2, 0, inner)
-    sc = max(1.0, math.sqrt(Sq / 64))
-    assert_close(dq, qr.grad, 3e-2, 3e-2, "attn dq")
-    assert_close(dkv1, k1r.grad, 3e-2, 3e-2 * sc, "attn dkv1")
-    if Sk2:
-        assert_close(dkv2, k2r.grad, 3e-2, 3e-2 * sc, "attn dkv2")
-
-
-@pytest.mark.parametrize("T,L,pos,attend_previous", [
-    (1, 256, [[0], [5]], True),
-    (2, 160, [[0, 40], [3, 90]], True),
-    (1, 64, [[0, 8, 16], [2, 9]], True),          # more <image> tokens than media -> uniform rows
-    (3, 300, [[0, 100, 200], [10, 20, 290]], False),
-    (2, 40, [[], [7]], True),                      # a sample without any <image>
-])
-def test_attention_media_mask(T, L, pos, attend_previous):
-    from oracle.restatement import text_time_np
-    from otter_b200 import functional as F
-    P, H, n = 2, 8, 64
-    inner = H * 64
-    loc = np.zeros((P, L), dtype=bool)
-    for b, ps in enumerate(pos):
-        loc[b, ps] = True
-    tt = F.text_time(torch.from_numpy(loc).to(dev()), attend_previous)
-    assert np.array_equal(tt.cpu().numpy().astype(np.int64), text_time_np(loc, attend_previous))
-    q = rnd(P * L, inner, seed=1)
-    kv = rnd(P * T * n, 2 * inner, seed=2)
-    spec = F.AttnSpec(q, 0, kv, 0, inner, P, H, L, T * n, 0.125, text_time=tt, n_per_media=n, T_img=T)
-    out, lse = F.attn_fwd(spec)
-    qr, kr = q.float().requires_grad_(True), kv.float().requires_grad_(True)
-    ref = _attn_ref(_heads(qr, P, L, H), _heads(kr[:, :inner], P, T * n, H), _heads(kr[:, inner:], P, T * n, H), 0.125,
-                    tt=tt.long(), n=n, T=T).permute(0, 2, 1, 3).reshape(P * L, inner)
-    assert_close(out, ref, 2e-2, 2e-2, "masked attn fwd")
-    # rows with text_time == 0 must be exactly zero
-    zero_rows = (tt.reshape(-1) == 0)
-    assert (out[zero_rows].float().abs().max().item() if zero_rows.any() else 0.0) == 0.0
-    dout = rnd(P * L, inner, seed=5)
-    ref.backward(dout.float())
-    dq, dkv = torch.zeros_like(q), torch.zeros_like(kv)
-    F.attn_bwd(spec, out, 0, lse, dout, 0, dq, 0, dkv, 0, inner)
-    assert_close(dq, qr.grad, 3e-2, 3e-2, "masked attn dq")
-    assert_close(dkv, kr.grad, 3e-2, 3e-2 * math.sqrt(L / 64), "masked attn dkv")
-
-
 def test_small_passes():
     from otter_b200 import functional as F
     src = torch.randn(64, 1024, device=dev())

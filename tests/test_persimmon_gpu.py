@@ -1,8 +1,7 @@
 """GPU: Persimmon decoder layer (SURVEY.md §8f rank 3) — the qk-LayerNorm + partial-RoPE kernels against plain torch,
-the causal mode of the fused attention kernels, and the whole layer fwd + bwd (every parameter gradient) against the
-CPU oracle pinned to HF Persimmon.  Production numerics (bf16 operands): tolerances of tests/test_modules_gpu.py."""
-import math
-
+and the whole layer fwd + bwd (every parameter gradient) against the CPU oracle pinned to HF Persimmon.  The causal
+mode of the head-64 attention kernels is tested in tests/test_attention_edges_gpu.py.
+Production numerics (bf16 operands): tolerances of tests/test_modules_gpu.py."""
 import pytest
 import torch
 
@@ -49,30 +48,6 @@ def test_qkln_rope_fwd_bwd_vs_torch(rows_S, H, rot):
     assert _rel(dfused, x.grad.reshape(rows, H * 192)) <= 1e-2
     for got, want in zip(grads, pr):
         assert _rel(got, want.grad) <= 1e-2, (_rel(got, want.grad))
-
-
-@pytest.mark.parametrize("P,H,S", [(2, 4, 100), (1, 2, 300), (2, 3, 520)])
-def test_causal_attention_fwd_bwd(P, H, S):
-    """causal flag of the head-64 kernels: S = 100 (resident kernel), 300 (3 key tiles), 520 (streaming kernel)."""
-    from otter_b200 import functional as F
-    g = torch.Generator().manual_seed(S)
-    D = H * 64
-    qkv = torch.randn(P * S, 3 * D, generator=g).to(BF16).to(DEV)
-    spec = F.AttnSpec(qkv, 0, qkv, D, 2 * D, P, H, S, S, 0.125, causal=True)
-    out, lse = F.attn_fwd(spec)
-    x = qkv.float().requires_grad_(True)
-    hd = lambda c: x[:, c * D:(c + 1) * D].reshape(P, S, H, 64).permute(0, 2, 1, 3)
-    sim = (hd(0) @ hd(1).transpose(-1, -2)) * 0.125
-    sim = sim.masked_fill(~torch.ones(S, S, dtype=torch.bool, device=DEV).tril(), float("-inf"))
-    ref = (sim.softmax(-1) @ hd(2)).permute(0, 2, 1, 3).reshape(P * S, D)
-    err = (out.float() - ref.detach()).abs()
-    assert (err > 2e-2 + 2e-2 * ref.detach().abs()).sum().item() == 0, err.max().item()
-    dout = torch.randn(P * S, D, generator=g).to(BF16).to(DEV)
-    ref.backward(dout.float())
-    dqkv = torch.zeros_like(qkv)
-    F.attn_bwd(spec, out, 0, lse, dout, 0, dqkv, 0, dqkv, D, 2 * D)
-    for c, name in enumerate(("dq", "dk", "dv")):
-        assert _rel(dqkv[:, c * D:(c + 1) * D], x.grad[:, c * D:(c + 1) * D]) <= 2e-2, name
 
 
 @pytest.mark.parametrize("B,S,D,H", [(2, 100, 256, 4), (1, 300, 512, 8)])
