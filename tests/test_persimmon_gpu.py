@@ -1,6 +1,6 @@
-"""GPU: Persimmon decoder layer (SURVEY.md §8f rank 3) — the qk-LayerNorm + partial-RoPE kernels against plain torch,
-and the whole layer fwd + bwd (every parameter gradient) against the CPU oracle pinned to HF Persimmon.  The causal
-mode of the head-64 attention kernels is tested in tests/test_attention_edges_gpu.py.
+"""GPU: Persimmon decoder layer (SURVEY.md §8f rank 3) — the whole layer fwd + bwd (every parameter gradient) against
+the CPU oracle pinned to HF Persimmon.  The causal mode of the head-64 attention kernels is tested in
+tests/test_attention_edges_gpu.py, the qk-LayerNorm + partial-RoPE kernels in tests/test_rowwise_edges_gpu.py.
 Production numerics (bf16 operands): tolerances of tests/test_modules_gpu.py."""
 import pytest
 import torch
@@ -15,39 +15,6 @@ BF16 = torch.bfloat16
 def _rel(got, ref):
     got, ref = got.detach().float().cpu(), ref.detach().float().cpu()
     return ((got - ref).norm() / ref.norm().clamp_min(1e-20)).item()
-
-
-@pytest.mark.parametrize("rows_S,H,rot", [((2, 37), 4, 32), ((1, 300), 2, 16), ((3, 8), 64, 32)])
-def test_qkln_rope_fwd_bwd_vs_torch(rows_S, H, rot):
-    from otter_b200 import functional as F
-    B, S = rows_S
-    rows = B * S
-    g = torch.Generator().manual_seed(rows + H)
-    fused = (torch.randn(rows, H * 192, generator=g) * 1.5).to(BF16)
-    par = [(1 + 0.2 * torch.randn(64, generator=g)), 0.2 * torch.randn(64, generator=g),
-           (1 + 0.2 * torch.randn(64, generator=g)), 0.2 * torch.randn(64, generator=g)]
-    qkv, stats = F.qkln_rope_fwd(fused.to(DEV), H, S, *[t.to(DEV) for t in par], rot, 25000.0, 1e-5)
-    # torch reference on the bf16-rounded input
-    x = fused.float().view(B, S, H, 3, 64).requires_grad_(True)
-    pr = [t.clone().requires_grad_(True) for t in par]
-    qs = RP.layer_norm(x[..., 0, :], pr[0], pr[1], 1e-5)
-    ks = RP.layer_norm(x[..., 1, :], pr[2], pr[3], 1e-5)
-    inv = 1.0 / (25000.0 ** (torch.arange(0, rot, 2, dtype=torch.float32) / rot))
-    fr = torch.arange(S, dtype=torch.float32)[:, None] * inv[None]
-    emb = torch.cat((fr, fr), -1)
-    cos, sin = emb.cos()[None, :, None, :], emb.sin()[None, :, None, :]
-    rope = lambda t: torch.cat((t[..., :rot] * cos + RP.rotate_half(t[..., :rot]) * sin, t[..., rot:]), -1)
-    ref = torch.cat([rope(qs).reshape(rows, H * 64), rope(ks).reshape(rows, H * 64), x[..., 2, :].reshape(rows, H * 64)], 1)
-    err = (qkv.float().cpu() - ref.detach()).abs()
-    assert (err > 2e-2 + 1e-2 * ref.detach().abs()).sum().item() == 0, err.max().item()
-    assert torch.equal(qkv[:, 2 * H * 64:].cpu(), fused.view(rows, H, 3, 64)[:, :, 2].reshape(rows, H * 64))   # v: copy
-    dq = torch.randn(rows, 3 * H * 64, generator=g).to(BF16)
-    ref.backward(dq.float())
-    grads = [torch.empty(64, device=DEV) for _ in range(4)]
-    dfused = F.qkln_rope_bwd(dq.to(DEV), fused.to(DEV), stats, H, S, par[0].to(DEV), par[2].to(DEV), rot, 25000.0, *grads)
-    assert _rel(dfused, x.grad.reshape(rows, H * 192)) <= 1e-2
-    for got, want in zip(grads, pr):
-        assert _rel(got, want.grad) <= 1e-2, (_rel(got, want.grad))
 
 
 @pytest.mark.parametrize("B,S,D,H", [(2, 100, 256, 4), (1, 300, 512, 8)])
