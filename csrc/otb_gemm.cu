@@ -438,6 +438,13 @@ extern "C" int otb_gemm_bf16(const void* A, int a_mn_major, int64_t lda, const v
   OTB_CHECK_ARG(A && B && e && e->out, "otb_gemm_bf16: null pointer");
   // the output tensor map of the TMA-store epilogue needs a 16-byte aligned base
   OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->out) & 15) == 0, "otb_gemm_bf16: out must be 16-byte aligned");
+  // the epilogue reads bias / residual / aux_in and writes aux_out in 16 B vectors
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->bias) & 15) == 0, "otb_gemm_bf16: bias must be 16-byte aligned");
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->residual) & 15) == 0,
+                "otb_gemm_bf16: residual must be 16-byte aligned");
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->aux_in) & 15) == 0, "otb_gemm_bf16: aux_in must be 16-byte aligned");
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(e->aux_out) & 15) == 0,
+                "otb_gemm_bf16: aux_out must be 16-byte aligned");
   OTB_CHECK_ARG(M > 0 && N > 0 && K > 0, "otb_gemm_bf16: bad shape %d %d %d", M, N, K);
   OTB_CHECK_ARG(N % 8 == 0, "otb_gemm_bf16: N=%d must be a multiple of 8", N);
   OTB_CHECK_ARG(e->ld_out % 8 == 0 && e->ld_out >= N, "otb_gemm_bf16: bad ld_out");

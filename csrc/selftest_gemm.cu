@@ -1,5 +1,5 @@
 // Standalone GPU self-test + micro-benchmark of otb_gemm_bf16 through the public C ABI.
-// Not part of the product path: a developer tool run under gpurun (see tests/test_gemm_gpu.py for the
+// Not part of the product path: a developer tool run by hand on an H100 (see tests/test_gemm_edges_gpu.py for the
 // pytest parity tests).  Reference = fp64 accumulation on the host over the bf16-rounded inputs.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

@@ -45,6 +45,18 @@ def test_invalid_arguments_return_error_codes():
     e.out, e.ld_out = 0x10002, 128
     rc = lib.otb_gemm_bf16(0x10000, 0, 128, 0x20000, 0, 128, 128, 128, 128, C.byref(e), None)
     assert rc == 1 and b"aligned" in lib.otb_last_error()
+    # bias / residual / aux_in / aux_out are read or written in 16 B vectors by the epilogue.  M = 0: the alignment
+    # check must come before the shape check, or the message below names the shape instead of the pointer.
+    launches = lib.otb_launch_count()
+    for name in ("bias", "residual", "aux_in", "aux_out"):
+        e = _lib.GemmEpilogue()
+        e.out, e.ld_out = 0x10000, 128
+        e.ld_aux_in = e.ld_aux_out = e.ld_res = 128
+        setattr(e, name, 0x30000 + 4)
+        rc = lib.otb_gemm_bf16(0x10000, 0, 128, 0x20000, 0, 128, 0, 128, 128, C.byref(e), None)
+        msg = lib.otb_last_error()
+        assert rc == 1 and name.encode() in msg and b"aligned" in msg, (name, msg)
+    assert lib.otb_launch_count() == launches
     assert lib.otb_text_time(None, 0, 0, 1, None, None) == 1
     assert lib.otb_layernorm_fwd(None, 0, None, None, None, 0, None, None, 0, 0, 1e-5, None) == 1
     d = _lib.AttnDesc()
