@@ -1,8 +1,9 @@
 // otter_b200 — causal self-attention of the frozen LM decoder layers (SURVEY.md §8f rank 1), head dim 128.
 //
-//   MPT-7B / LLaMA-7B shape: 32 heads x 128, S = L (256 ... 2048), Q/K/V read in place from the fused Wqkv GEMM output
-//   ([B*S][3*D] bf16, head h at columns col0 + h*128), optional ALiBi key bias slope_h * (j - (S-1)) added to the
-//   scaled scores (mpt/attention.py:51-56,457-464), causal mask (mpt/attention.py:68-75).
+//   MPT-7B / LLaMA shapes: H query heads x 128, S = L (256 ... 2048), Q/K/V read in place from the fused Wqkv GEMM
+//   output (bf16, head h at columns col0 + h*128), optional ALiBi key bias slope_h * (j - (S-1)) added to the scaled
+//   scores (mpt/attention.py:51-56,457-464), causal mask (mpt/attention.py:68-75).  Grouped-query attention
+//   (Llama-2-70B, Llama-3): kv_heads K/V heads, query head h reads K/V head h / (H / kv_heads) (HF's repeat_kv).
 //
 // Same machinery as otb_attn.cu (wgmma from 128B-swizzled TMA tiles, one warpgroup, softmax rows owned by threads and
 // read from swizzled fp32 smem tiles), with every 128-wide operand held as two 64-column SW128 panels:
@@ -13,6 +14,9 @@
 //            tiles: for key tile j, for query tile i that sees it: S, dP = dO V^T, P / dS staged in smem, dV_j += P^T dO,
 //            dK_j += dS^T Q, dQ_i = dS K_j through a 64 KB fp32 tile and accumulated across key tiles in an fp32
 //            workspace.  The weights of the LM are frozen: there is no wgrad, only these activation gradients.
+//            With a group of g = H / kv_heads > 1 query heads per K/V head, each CTA still owns one query head: it writes
+//            its fp32 dK/dV partials to the workspace and lm_attn_kv_reduce_kernel sums the g partials of a K/V head in
+//            a fixed order (deterministic, no atomics; H*B CTAs instead of kv_heads*B).
 #include "otb_common.cuh"
 #include "otb_host.h"
 
@@ -28,6 +32,7 @@ constexpr float kLog2e = 1.4426950408889634f;
 struct LmAttnParams {
   int B, H, S, causal;
   int q_col0, k_col0, v_col0;
+  int kv_group;                          // H / kv_heads: query head h reads K/V head h / kv_group
   float scale, scale_log2;
   const float* slopes;                   // [H] ALiBi slopes or nullptr
   bf16* out; long long ldo; int o_col0;
@@ -35,6 +40,7 @@ struct LmAttnParams {
   const bf16* dout; long long ld_do; int do_col0;
   bf16* dqkv; long long ld_dqkv; int dq_col0, dk_col0, dv_col0;
   float* dq_ws;                          // [B*S][H*128] fp32
+  float* dk_ws; float* dv_ws;            // kv_group > 1: per-query-head dK / dV partials, [B*S][H*128] fp32 each
 };
 
 __device__ __forceinline__ float lm_ex2(float x) {
@@ -73,6 +79,7 @@ lm_attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, LmAttnParams p) 
 
   const int tid = threadIdx.x;
   const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int kvh = h / p.kv_group;
 
   if (tid == 0) {
     mbar_init(&full[0], 1); mbar_init(&full[1], 1); mbar_init(bar_q, 1);
@@ -97,8 +104,8 @@ lm_attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, LmAttnParams p) 
     mbar_arrive_expect_tx(&full[st], need_v ? 2 * kTile2 : kTile2);
 #pragma unroll
     for (int pp = 0; pp < 2; ++pp) {
-      tma_load_2d(s_k + st * kTile2 + pp * kPanel, &map_qkv, &full[st], p.k_col0 + h * 128 + pp * 64, krow);
-      if (need_v) tma_load_2d(s_v + st * kTile2 + pp * kPanel, &map_qkv, &full[st], p.v_col0 + h * 128 + pp * 64, krow);
+      tma_load_2d(s_k + st * kTile2 + pp * kPanel, &map_qkv, &full[st], p.k_col0 + kvh * 128 + pp * 64, krow);
+      if (need_v) tma_load_2d(s_v + st * kTile2 + pp * kPanel, &map_qkv, &full[st], p.v_col0 + kvh * 128 + pp * 64, krow);
     }
   };
   const uint32_t q_addr = smem_u32(s_q), p_addr = smem_u32(s_p);
@@ -230,6 +237,9 @@ lm_attn_fwd_kernel(const __grid_constant__ CUtensorMap map_qkv, LmAttnParams p) 
 // ================================================================================================
 // backward (activation gradients only)
 // ================================================================================================
+// kGrouped: dK / dV partials of this query head go to p.dk_ws / p.dv_ws in fp32 (summed by lm_attn_kv_reduce_kernel);
+// otherwise they are final and written to dqkv in bf16.
+template <bool kGrouped>
 __global__ void __launch_bounds__(kLmThreads)
 lm_attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant__ CUtensorMap map_kv,
                    const __grid_constant__ CUtensorMap map_do, LmAttnParams p) {
@@ -250,6 +260,7 @@ lm_attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
 
   const int tid = threadIdx.x;
   const int h = blockIdx.x, b = blockIdx.y;
+  const int kvh = h / p.kv_group;
 
   if (tid == 0) {
     mbar_init(bar_kv, 1); mbar_init(bar_qdo, 1);
@@ -274,8 +285,8 @@ lm_attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
       mbar_arrive_expect_tx(bar_kv, 4 * kKPanel);
 #pragma unroll
       for (int pp = 0; pp < 2; ++pp) {
-        tma_load_2d(s_k + pp * kKPanel, &map_kv, bar_kv, p.k_col0 + h * 128 + pp * 64, krow);
-        tma_load_2d(s_v + pp * kKPanel, &map_kv, bar_kv, p.v_col0 + h * 128 + pp * 64, krow);
+        tma_load_2d(s_k + pp * kKPanel, &map_kv, bar_kv, p.k_col0 + kvh * 128 + pp * 64, krow);
+        tma_load_2d(s_v + pp * kKPanel, &map_kv, bar_kv, p.v_col0 + kvh * 128 + pp * 64, krow);
       }
     }
     float dv[1][64], dk[1][64];      // dV_j, dK_j: the 64 keys of this tile x 128 d
@@ -425,6 +436,14 @@ lm_attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
           if (key_ok) {
             uint32_t r[32];
             acc_ld32<128>(src, tid, c * 32, r);
+            if constexpr (kGrouped) {
+              float* dst = (w ? p.dk_ws : p.dv_ws) + static_cast<long long>(krow + tid) * (p.H * 128) + h * 128 + c * 32;
+#pragma unroll
+              for (int e = 0; e < 32; e += 4)
+                *reinterpret_cast<float4*>(dst + e) = make_float4(__uint_as_float(r[e]), __uint_as_float(r[e + 1]),
+                                                                  __uint_as_float(r[e + 2]), __uint_as_float(r[e + 3]));
+              continue;
+            }
             bf16* dst = p.dqkv + static_cast<long long>(krow + tid) * p.ld_dqkv + (w ? p.dk_col0 : p.dv_col0) + h * 128 +
                         c * 32;
 #pragma unroll
@@ -444,6 +463,35 @@ lm_attn_bwd_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_const
   }
 }
 
+// dK / dV of K/V head kvh = sum over r = 0 .. kv_group-1 (in this order) of the partials of query head kvh*kv_group + r.
+// Thread = 8 columns of one (row, dK or dV, K/V head).
+__global__ void __launch_bounds__(256) lm_attn_kv_reduce_kernel(LmAttnParams p) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int nkv = p.H / p.kv_group;
+  const long long total = static_cast<long long>(p.B) * p.S * 2 * nkv * 16;
+  for (long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; idx < total;
+       idx += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int u = static_cast<int>(idx & 15);
+    const long long t = idx >> 4;
+    const int kvh = static_cast<int>(t % nkv);
+    const long long t2 = t / nkv;
+    const int w = static_cast<int>(t2 & 1);               // 0: dV, 1: dK
+    const long long row = t2 >> 1;
+    const float* src = (w ? p.dk_ws : p.dv_ws) + row * (p.H * 128) + kvh * p.kv_group * 128 + u * 8;
+    float a[8];
+    {
+      const float4 x0 = reinterpret_cast<const float4*>(src)[0], x1 = reinterpret_cast<const float4*>(src)[1];
+      a[0] = x0.x; a[1] = x0.y; a[2] = x0.z; a[3] = x0.w; a[4] = x1.x; a[5] = x1.y; a[6] = x1.z; a[7] = x1.w;
+    }
+    for (int r = 1; r < p.kv_group; ++r) {
+      const float4 x0 = reinterpret_cast<const float4*>(src + r * 128)[0], x1 = reinterpret_cast<const float4*>(src + r * 128)[1];
+      a[0] += x0.x; a[1] += x0.y; a[2] += x0.z; a[3] += x0.w; a[4] += x1.x; a[5] += x1.y; a[6] += x1.z; a[7] += x1.w;
+    }
+    *reinterpret_cast<uint4*>(p.dqkv + row * p.ld_dqkv + (w ? p.dk_col0 : p.dv_col0) + kvh * 128 + u * 8) = pack8(a);
+  }
+}
+
 constexpr int kLmFwdSmem = 6 * kTile2 + kTile2 + 1024 + 128;
 constexpr int kLmBwdSmem = 4 * kKPanel + 2 * kTile2 + 2 * kPanel + 2 * kTile2 + 1024 + 128;
 
@@ -454,7 +502,9 @@ using namespace otb;
 static int lm_check(const otb_lm_attn_desc* d) {
   OTB_CHECK_ARG(d != nullptr && d->qkv != nullptr && d->out != nullptr, "otb_lm_attn: null pointer");
   OTB_CHECK_ARG(d->B > 0 && d->H > 0 && d->S > 0, "otb_lm_attn: bad sizes");
-  OTB_CHECK_ARG(d->head_dim == 128, "otb_lm_attn: head_dim must be 128 (MPT-7B / LLaMA-7B)");
+  OTB_CHECK_ARG(d->head_dim == 128, "otb_lm_attn: head_dim must be 128 (MPT-7B / LLaMA)");
+  OTB_CHECK_ARG(d->kv_heads >= 0 && (d->kv_heads == 0 || d->H % d->kv_heads == 0),
+                "otb_lm_attn: kv_heads must divide H (0 means H)");
   OTB_CHECK_ARG(d->ld_qkv % 8 == 0 && d->ld_out % 8 == 0, "otb_lm_attn: row pitches must be multiples of 8");
   OTB_CHECK_ARG(d->q_col0 % 8 == 0 && d->k_col0 % 8 == 0 && d->v_col0 % 8 == 0 && d->out_col0 % 8 == 0,
                 "otb_lm_attn: column offsets must be multiples of 8");
@@ -464,13 +514,14 @@ static int lm_check(const otb_lm_attn_desc* d) {
 static void lm_fill(const otb_lm_attn_desc* d, LmAttnParams& p) {
   p.B = d->B; p.H = d->H; p.S = d->S; p.causal = d->causal;
   p.q_col0 = d->q_col0; p.k_col0 = d->k_col0; p.v_col0 = d->v_col0;
+  p.kv_group = d->kv_heads ? d->H / d->kv_heads : 1;
   p.scale = d->scale; p.scale_log2 = d->scale * kLog2e;
   p.slopes = d->alibi_slopes;
   p.out = static_cast<bf16*>(d->out); p.ldo = d->ld_out; p.o_col0 = d->out_col0;
   p.lse = d->lse;
   p.dout = nullptr; p.ld_do = 0; p.do_col0 = 0;
   p.dqkv = nullptr; p.ld_dqkv = 0; p.dq_col0 = p.dk_col0 = p.dv_col0 = 0;
-  p.dq_ws = nullptr;
+  p.dq_ws = p.dk_ws = p.dv_ws = nullptr;
 }
 
 extern "C" int otb_lm_attn_fwd(const otb_lm_attn_desc* d, void* stream) {
@@ -494,6 +545,8 @@ extern "C" int otb_lm_attn_bwd(const otb_lm_attn_desc* d, const otb_lm_attn_grad
   if (rc) return rc;
   OTB_CHECK_ARG(g && d->lse && g->dout && g->dqkv, "otb_lm_attn_bwd: null tensor");
   OTB_CHECK_ARG(d->S <= kBwdKeys || g->dq_ws != nullptr, "otb_lm_attn_bwd: dq workspace required for S > 64");
+  OTB_CHECK_ARG(d->kv_heads == 0 || d->kv_heads == d->H || g->dq_ws != nullptr,
+                "otb_lm_attn_bwd: workspace required when kv_heads < H");
   OTB_CHECK_ARG(g->ld_dout % 8 == 0 && g->ld_dqkv % 8 == 0, "otb_lm_attn_bwd: row pitches must be multiples of 8");
   LmAttnParams p;
   lm_fill(d, p);
@@ -501,6 +554,12 @@ extern "C" int otb_lm_attn_bwd(const otb_lm_attn_desc* d, const otb_lm_attn_grad
   p.dqkv = static_cast<bf16*>(g->dqkv); p.ld_dqkv = g->ld_dqkv;
   p.dq_col0 = g->dq_col0; p.dk_col0 = g->dk_col0; p.dv_col0 = g->dv_col0;
   p.dq_ws = g->dq_ws;
+  const bool grouped = p.kv_group > 1;
+  if (grouped) {                         // [3][B*S][H*128]: dQ, dK partials, dV partials
+    const long long plane = static_cast<long long>(d->B) * d->S * d->H * 128;
+    p.dk_ws = g->dq_ws + plane;
+    p.dv_ws = g->dq_ws + 2 * plane;
+  }
   CUtensorMap mq, mkv, mdo;
   rc = make_tmap_bf16_2d(&mq, d->qkv, (uint64_t)d->B * d->S, d->qkv_cols, d->ld_qkv, 128, 64);
   if (rc) return rc;
@@ -508,11 +567,19 @@ extern "C" int otb_lm_attn_bwd(const otb_lm_attn_desc* d, const otb_lm_attn_grad
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&mdo, g->dout, (uint64_t)d->B * d->S, g->dout_cols, g->ld_dout, 128, 64);
   if (rc) return rc;
-  OTB_CHECK_CUDA(ensure_dyn_smem(lm_attn_bwd_kernel, kLmBwdSmem));
+  const auto kernel = grouped ? lm_attn_bwd_kernel<true> : lm_attn_bwd_kernel<false>;
+  OTB_CHECK_CUDA(ensure_dyn_smem(kernel, kLmBwdSmem));
   dim3 grid(d->H, d->B);
-  OTB_CHECK_CUDA(launch_k(lm_attn_bwd_kernel, grid, dim3(kLmThreads), kLmBwdSmem, static_cast<cudaStream_t>(stream), mq, mkv,
-                          mdo, p));
+  OTB_CHECK_CUDA(launch_k(kernel, grid, dim3(kLmThreads), kLmBwdSmem, static_cast<cudaStream_t>(stream), mq, mkv, mdo, p));
   count_launch();
   OTB_CHECK_CUDA(cudaGetLastError());
+  if (grouped) {
+    const long long units = static_cast<long long>(d->B) * d->S * 2 * (d->H / p.kv_group) * 16;
+    const long long cap = static_cast<long long>(sm_count()) * 8;
+    const int blocks = static_cast<int>(std::min((units + 255) / 256, cap));
+    OTB_CHECK_CUDA(launch_k(lm_attn_kv_reduce_kernel, dim3(blocks), dim3(256), 0, static_cast<cudaStream_t>(stream), p));
+    count_launch();
+    OTB_CHECK_CUDA(cudaGetLastError());
+  }
   return OTB_OK;
 }

@@ -1,9 +1,11 @@
-// otter_b200 — LLaMA decoder-layer specific kernels (SURVEY.md §8f rank 1, the LLaMA-7B text model of OTTER-Video / c3).
+// otter_b200 — LLaMA decoder-layer specific kernels (SURVEY.md §8f rank 1: the LLaMA-7B text model of OTTER-Video / c3,
+// and the grouped-query / scaled-RoPE LLaMA layers of Llama-2-70B and Llama-3).
 //   reference: xformers_model/llama.py:74-89 (LlamaRMSNorm), :150-166 (rotate_half / apply_rotary_pos_emb),
 //              :169-185 (LlamaMLP: down(silu(gate(x)) * up(x))), :186-259 (attention), :262-320 (decoder layer)
 // HBM-bound element-wise passes around the wgmma GEMMs and the head-dim-128 causal attention kernel:
 //   rmsnorm fwd / bwd(dx)     y = x * rsqrt(mean(x^2) + eps) * w             (the LM is frozen: no weight gradient)
-//   rope (in place)           q, k columns of the [rows][3*D] projection buffer, rotate_half convention, head dim 128
+//   rope (in place)           q, k columns of the fused projection buffer, rotate_half convention, head dim 128;
+//                             frequencies from theta, or from a table (linear / llama3 / yarn scaling) with a cos/sin factor
 //   swiglu fwd / bwd          h = silu(g) * u ;  dg = dh * u * silu'(g), du = dh * silu(g)
 #include "otb_common.cuh"
 #include "otb_host.h"
@@ -87,9 +89,12 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __re
 
 // In-place rotary embedding of `nblk` column blocks of H heads x 128 dims (q and k of the fused projection buffer).
 // Thread = one (row, block, head, pair index i < 64): x_i' = x_i c - x_{i+64} s ; x_{i+64}' = x_{i+64} c + x_i s
-// (rotate_half), angle = pos * theta^(-2i/128); sign = -1 applies the transpose (backward).
+// (rotate_half), angle = pos * inv_freq_i with inv_freq_i = theta^(-2i/128), or inv_tab[i] when a table is given (scaled
+// RoPE); c, s are multiplied by attn_scale (yarn's attention factor, 1 otherwise); sign = -1 applies the transpose
+// (backward).
 __global__ void __launch_bounds__(256)
-rope128_kernel(bf16* __restrict__ buf, long long ld, long long rows, int H, int S, int nblk, float log2_theta, float sign) {
+rope128_kernel(bf16* __restrict__ buf, long long ld, long long rows, int H, int S, int nblk, float log2_theta,
+               const float* __restrict__ inv_tab, float attn_scale, float sign) {
   pdl_launch_dependents();
   pdl_wait();
   const long long total = rows * nblk * H * 64;
@@ -102,10 +107,11 @@ rope128_kernel(bf16* __restrict__ buf, long long ld, long long rows, int H, int 
     const int blk = static_cast<int>(t2 % nblk);
     const long long row = t2 / nblk;
     const int pos = static_cast<int>(row % S);
-    const float inv_freq = exp2f(-log2_theta * static_cast<float>(2 * i) / 128.0f);
+    const float inv_freq = inv_tab != nullptr ? __ldg(inv_tab + i) : exp2f(-log2_theta * static_cast<float>(2 * i) / 128.0f);
     float s, c;
     sincosf(static_cast<float>(pos) * inv_freq, &s, &c);
-    s *= sign;
+    c *= attn_scale;
+    s *= sign * attn_scale;
     bf16* p = buf + row * ld + (static_cast<long long>(blk) * H + h) * 128 + i;
     const float a = __bfloat162float(p[0]), b = __bfloat162float(p[64]);
     p[0] = __float2bfloat16_rn(a * c - b * s);
@@ -202,7 +208,20 @@ extern "C" int otb_rope128(void* buf, int64_t ld, int64_t rows, int H, int S, in
   OTB_CHECK_ARG(buf && rows > 0 && H > 0 && S > 0 && nblk > 0 && ld >= (int64_t)nblk * H * 128 && rope_theta > 1.f,
                 "otb_rope128: bad argument");
   OTB_CHECK_CUDA(launch_k(rope128_kernel, dim3(ew_grid(rows * nblk * H * 64)), dim3(256), 0, ST(stream), static_cast<bf16*>(buf),
-                          (long long)ld, (long long)rows, H, S, nblk, log2f(rope_theta), backward ? -1.0f : 1.0f));
+                          (long long)ld, (long long)rows, H, S, nblk, log2f(rope_theta), static_cast<const float*>(nullptr),
+                          1.0f, backward ? -1.0f : 1.0f));
+  count_launch();
+  OTB_CHECK_CUDA(cudaGetLastError());
+  return OTB_OK;
+}
+
+extern "C" int otb_rope128_freqs(void* buf, int64_t ld, int64_t rows, int H, int S, int nblk, const float* inv_freq,
+                                 float attn_scale, int backward, void* stream) {
+  OTB_CHECK_ARG(buf && inv_freq && rows > 0 && H > 0 && S > 0 && nblk > 0 && ld >= (int64_t)nblk * H * 128 &&
+                    attn_scale > 0.f && attn_scale < INFINITY,
+                "otb_rope128_freqs: bad argument");
+  OTB_CHECK_CUDA(launch_k(rope128_kernel, dim3(ew_grid(rows * nblk * H * 64)), dim3(256), 0, ST(stream), static_cast<bf16*>(buf),
+                          (long long)ld, (long long)rows, H, S, nblk, 0.0f, inv_freq, attn_scale, backward ? -1.0f : 1.0f));
   count_launch();
   OTB_CHECK_CUDA(cudaGetLastError());
   return OTB_OK;

@@ -144,13 +144,16 @@ int otb_xattn_out_fused(const otb_attn_desc* d, const void* wo, int64_t ld_wo, c
                         int64_t ld_res, void* aux, int64_t ld_aux, void* y, int64_t ld_y, int D, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * SURVEY.md §8f rank 1 — causal self-attention of the frozen LM decoder layers (head_dim 128: MPT-7B / LLaMA-7B).
+ * SURVEY.md §8f rank 1 — causal self-attention of the frozen LM decoder layers (head_dim 128: MPT-7B / LLaMA).
  *   mpt/attention.py:22-84 (scaled_multihead_dot_product_attention), :457-464 (ALiBi key bias), :68-75 (causal mask)
  * qkv is the fused Wqkv GEMM output [B*S][qkv_cols] bf16 (row pitch ld_qkv): head h of Q / K / V at columns
  * q_col0 / k_col0 / v_col0 + h*128.  out [B*S][..] bf16, head h at out_col0 + h*128; lse fp32 [B][H][S].
  *   score(i,j) = scale * q_i.k_j + alibi_slopes[h] * (j - (S-1))      (alibi_slopes NULL: no bias)
  *   causal != 0: keys j > i are masked.
- * Backward returns activation gradients only (the LM is frozen): dqkv has the layout of qkv.
+ * kv_heads: number of K/V heads (grouped-query attention; 0 means H).  H % kv_heads must be 0; query head h reads K/V
+ *   head h / (H / kv_heads) at k_col0 / v_col0 + that*128 (HF's repeat_kv).  lse stays one row per query head.
+ * Backward returns activation gradients only (the LM is frozen): dqkv has the layout of qkv; with kv_heads < H, dK / dV
+ *   of a K/V head are the sum over its query heads, reduced in a fixed order (deterministic).
  * ------------------------------------------------------------------------------------------- */
 typedef struct otb_lm_attn_desc {
   const void* qkv;
@@ -161,12 +164,14 @@ typedef struct otb_lm_attn_desc {
   int32_t qkv_cols, q_col0, k_col0, v_col0, out_col0;
   int32_t B, H, S, head_dim, causal;
   float scale;
+  int32_t kv_heads;          /* 0 = H; occupies what was the struct's tail padding: sizeof stays 96 */
 } otb_lm_attn_desc;
 
 typedef struct otb_lm_attn_grads {
   const void* dout; /* [B*S][dout_cols] bf16, head h at dout_col0 + h*128 */
   void* dqkv;       /* [B*S][..] bf16: dQ / dK / dV of head h at dq_col0 / dk_col0 / dv_col0 + h*128 */
-  float* dq_ws;     /* fp32 [B*S][H*128] scratch, required when S > 64 (the backward walks 64-key tiles) */
+  float* dq_ws;     /* fp32 [B*S][H*128] scratch, required when S > 64 (the backward walks 64-key tiles);
+                       with kv_heads < H: fp32 [3][B*S][H*128] (dQ, dK and dV partials per query head), always required */
   int64_t ld_dout, ld_dqkv;
   int32_t dout_cols, dout_col0, dq_col0, dk_col0, dv_col0;
   int32_t _pad;
@@ -283,12 +288,17 @@ int otb_fuyu_scatter(const void* word, const void* cont, const int64_t* idx, con
  *   otb_rmsnorm_bwd   dx (+ add) — the LM is frozen, no weight gradient
  *   otb_rope128       in place on `nblk` column blocks of H heads x 128 (q and k of a [rows][3*H*128] buffer); position of
  *                     a row = row % S; backward != 0 applies the transposed rotation
+ *   otb_rope128_freqs the same rotation with inv_freq fp32 [64] from a table (HF's linear / llama3 / yarn RoPE scaling)
+ *                     and cos / sin multiplied by attn_scale (yarn's attention factor; 1 otherwise).  With grouped-query
+ *                     attention the q block (H heads) and the k block (kv_heads heads) are two calls on column slices
  *   otb_swiglu_fwd/bwd  h = silu(g) * u ; dg, du from dh.   All bf16, row pitches in elements (multiples of 8). */
 int otb_rmsnorm_fwd(const void* x, int64_t ldx, const float* weight, void* y, int64_t ldy, float* rstd, int rows, int D,
                     float eps, void* stream);
 int otb_rmsnorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* rstd, const float* weight,
                     const void* add, int64_t ldadd, void* dx, int64_t lddx, int rows, int D, void* stream);
 int otb_rope128(void* buf, int64_t ld, int64_t rows, int H, int S, int nblk, float rope_theta, int backward, void* stream);
+int otb_rope128_freqs(void* buf, int64_t ld, int64_t rows, int H, int S, int nblk, const float* inv_freq, float attn_scale,
+                      int backward, void* stream);
 int otb_swiglu_fwd(const void* g, int64_t ldg, const void* u, int64_t ldu, void* h, int64_t ldh, int64_t rows, int I,
                    void* stream);
 int otb_swiglu_bwd(const void* dh, int64_t lddh, const void* g, int64_t ldg, const void* u, int64_t ldu, void* dg,

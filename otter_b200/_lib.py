@@ -55,7 +55,7 @@ class LmAttnDesc(C.Structure):
         ("qkv_cols", C.c_int32), ("q_col0", C.c_int32), ("k_col0", C.c_int32), ("v_col0", C.c_int32),
         ("out_col0", C.c_int32),
         ("B", C.c_int32), ("H", C.c_int32), ("S", C.c_int32), ("head_dim", C.c_int32), ("causal", C.c_int32),
-        ("scale", C.c_float),
+        ("scale", C.c_float), ("kv_heads", C.c_int32),
     ]
 
 
@@ -117,6 +117,7 @@ SIGNATURES = {
     "otb_rmsnorm_fwd": (_I, [_VP, _I64, _VP, _VP, _I64, _VP, _I, _I, _F, _VP]),
     "otb_rmsnorm_bwd": (_I, [_VP, _I64, _VP, _I64, _VP, _VP, _VP, _I64, _VP, _I64, _I, _I, _VP]),
     "otb_rope128": (_I, [_VP, _I64, _I64, _I, _I, _I, _F, _I, _VP]),
+    "otb_rope128_freqs": (_I, [_VP, _I64, _I64, _I, _I, _I, _VP, _F, _I, _VP]),
     "otb_swiglu_fwd": (_I, [_VP, _I64, _VP, _I64, _VP, _I64, _I64, _I, _VP]),
     "otb_swiglu_bwd": (_I, [_VP, _I64, _VP, _I64, _VP, _I64, _VP, _I64, _VP, _I64, _I64, _I, _VP]),
     "otb_qkln_rope_ws_floats": (_I, []),

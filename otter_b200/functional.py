@@ -155,45 +155,60 @@ def linear_wgrad(dy, x, *, out=None, accumulate=False, **epi):
 # ------------------------------------------------------------------------------------------------
 # Causal self-attention of the frozen LM layers (head dim 128) — SURVEY.md §8f rank 1
 # ------------------------------------------------------------------------------------------------
-def _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale):
+def _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale, kv_heads):
     d = LmAttnDesc()
     d.qkv, d.out, d.lse, d.alibi_slopes = _p(qkv), _p(out), _p(lse), _p(slopes)
     d.ld_qkv, d.ld_out = qkv.stride(0), out.stride(0)
-    D = H * 128
-    d.qkv_cols, d.q_col0, d.k_col0, d.v_col0, d.out_col0 = qkv.shape[1], 0, D, 2 * D, 0
+    D, Dkv = H * 128, kv_heads * 128
+    d.qkv_cols, d.q_col0, d.k_col0, d.v_col0, d.out_col0 = qkv.shape[1], 0, D, D + Dkv, 0
     d.B, d.H, d.S, d.head_dim, d.causal = B, H, S, 128, 1 if causal else 0
     d.scale = scale
+    d.kv_heads = kv_heads
     return d
 
 
+def _kv_heads(H, kv_heads):
+    kv = H if kv_heads is None else int(kv_heads)
+    if kv <= 0 or H % kv != 0:
+        raise _lib.OtbError(f"kv_heads = {kv_heads} must divide the {H} query heads")
+    return kv
+
+
 @_on_device
-def lm_attn_fwd(qkv, B, S, H, *, slopes=None, causal=True, scale=None):
-    """qkv bf16 [B*S, 3*H*128] (fused Wqkv output, [q|k|v]) -> (out bf16 [B*S, H*128], lse fp32 [B, H, S])."""
+def lm_attn_fwd(qkv, B, S, H, *, slopes=None, causal=True, scale=None, kv_heads=None):
+    """qkv bf16 [B*S, (H + 2*kv_heads)*128] (fused Wqkv output, [q|k|v]; kv_heads K/V heads for grouped-query
+    attention, default H) -> (out bf16 [B*S, H*128], lse fp32 [B, H, S])."""
     qkv = _mat(qkv, "qkv")
-    assert qkv.shape == (B * S, 3 * H * 128), qkv.shape
+    kv_heads = _kv_heads(H, kv_heads)
+    assert qkv.shape == (B * S, (H + 2 * kv_heads) * 128), qkv.shape
     if slopes is not None:
         _req(slopes, torch.float32, "alibi slopes")
     out = torch.empty((B * S, H * 128), device=qkv.device, dtype=BF16)
     lse = torch.empty((B, H, S), device=qkv.device, dtype=torch.float32)
     scale = (128 ** -0.5) if scale is None else scale
-    d = _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale)
+    d = _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale, kv_heads)
     check(_lib.load().otb_lm_attn_fwd(C.byref(d), _stream()), "otb_lm_attn_fwd")
     return out, lse
 
 
 @_on_device
-def lm_attn_bwd(dout, qkv, out, lse, B, S, H, *, slopes=None, causal=True, scale=None):
-    """-> dqkv bf16 [B*S, 3*H*128] ([dq|dk|dv], the layout of qkv)."""
+def lm_attn_bwd(dout, qkv, out, lse, B, S, H, *, slopes=None, causal=True, scale=None, kv_heads=None):
+    """-> dqkv bf16 with the layout of qkv ([dq|dk|dv]).  With kv_heads < H, dK / dV of a K/V head are summed over its
+    query heads in a fixed order (deterministic)."""
     dout, qkv, out = _mat(dout, "dout"), _mat(qkv, "qkv"), _mat(out, "out")
     scale = (128 ** -0.5) if scale is None else scale
-    d = _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale)
+    kv_heads = _kv_heads(H, kv_heads)
+    d = _lm_desc(qkv, out, lse, slopes, B, S, H, causal, scale, kv_heads)
     dqkv = torch.empty_like(qkv)
     g = LmAttnGrads()
-    ws = torch.empty((B * S, H * 128), device=qkv.device, dtype=torch.float32) if S > 64 else None
-    D = H * 128
+    if kv_heads < H:          # dQ, then the per-query-head dK and dV partials
+        ws = torch.empty((3, B * S, H * 128), device=qkv.device, dtype=torch.float32)
+    else:
+        ws = torch.empty((B * S, H * 128), device=qkv.device, dtype=torch.float32) if S > 64 else None
+    D, Dkv = H * 128, kv_heads * 128
     g.dout, g.dqkv, g.dq_ws = _p(dout), _p(dqkv), _p(ws)
     g.ld_dout, g.ld_dqkv = dout.stride(0), dqkv.stride(0)
-    g.dout_cols, g.dout_col0, g.dq_col0, g.dk_col0, g.dv_col0 = dout.shape[1], 0, 0, D, 2 * D
+    g.dout_cols, g.dout_col0, g.dq_col0, g.dk_col0, g.dv_col0 = dout.shape[1], 0, 0, D, D + Dkv
     check(_lib.load().otb_lm_attn_bwd(C.byref(d), C.byref(g), _stream()), "otb_lm_attn_bwd")
     return dqkv
 
@@ -522,6 +537,19 @@ def rope128_(buf, H, S, nblk, rope_theta, backward=False):
     buf = _mat(buf, "buf")
     check(_lib.load().otb_rope128(_p(buf), buf.stride(0), buf.shape[0], H, S, nblk, float(rope_theta), int(bool(backward)),
                                   _stream()), "otb_rope128")
+    return buf
+
+
+@_on_device
+def rope128_freqs_(buf, H, S, nblk, inv_freq, attn_scale=1.0, backward=False):
+    """In place: rotary embedding as rope128_, with the inverse frequencies from inv_freq (fp32 [64], on the device:
+    HF's linear / llama3 / yarn scaled RoPE) and cos / sin multiplied by attn_scale."""
+    buf = _mat(buf, "buf")
+    _req(inv_freq, torch.float32, "inv_freq")
+    if inv_freq.shape != (64,) or inv_freq.device != buf.device:
+        raise _lib.OtbError(f"inv_freq must be fp32 [64] on {buf.device}, got {tuple(inv_freq.shape)} on {inv_freq.device}")
+    check(_lib.load().otb_rope128_freqs(_p(buf), buf.stride(0), buf.shape[0], H, S, nblk, _p(inv_freq), float(attn_scale),
+                                        int(bool(backward)), _stream()), "otb_rope128_freqs")
     return buf
 
 

@@ -5,10 +5,14 @@ Mirrors `LlamaDecoderLayer` (/root/reference/xformers_model/llama.py:262-320; th
 (`input_layernorm`, `self_attn.{q,k,v,o}_proj`, `post_attention_layernorm`, `mlp.{gate,up,down}_proj`), no biases.
 The layer is FROZEN in Otter (modeling_otter.py:897-905): backward produces the input gradient only.
 
-  RMSNorm -> q / k / v GEMMs into one [rows, 3D] buffer -> rotary embedding in place (rotate_half, head dim 128)
-     -> causal attention (otb_lm_attn_*, no key bias) -> o_proj GEMM (+residual)
+  RMSNorm -> q / k / v GEMMs into one [rows, (H + 2 kv) * 128] buffer -> rotary embedding in place (rotate_half,
+     head dim 128) -> causal attention (otb_lm_attn_*, no key bias) -> o_proj GEMM (+residual)
      -> RMSNorm -> gate / up GEMMs -> silu(g) * u -> down GEMM (+residual)
 head_dim must be 128 (LLaMA-7B: 4096 = 32 x 128); training path (no KV cache); default position ids.
+Grouped-query attention (kv < H K/V heads: Llama-2-70B, Llama-3) and the linear / llama3 / yarn RoPE scalings are
+covered too: the RoPE table (inverse frequencies and yarn's cos / sin factor) comes from HF's own LlamaRotaryEmbedding,
+so none of the scaling formulas is restated here.  `dynamic` and `longrope` depend on the sequence length at run time
+and are not covered.
 `swap_llama_layers(model)` replaces the decoder layers of an HF `LlamaForCausalLM` by this class, sharing the Parameter
 objects.  Attention masks: the kernel applies the causal mask only, which equals HF's causal + padding mask at every
 non-pad position when padding is on the RIGHT (the training collate, SURVEY.md §8f-2); a forward pre-hook on the LlamaModel
@@ -31,15 +35,17 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
     def forward(ctx, x, layer, B, S):
         a, m = layer.self_attn, layer.mlp
         D, H = layer.hidden_size, layer.num_heads
+        Dkv = layer.num_key_value_heads * 128
         x2 = x.reshape(B * S, D)
         w_in, w_post = P.f32_of(layer.input_layernorm.weight), P.f32_of(layer.post_attention_layernorm.weight)
         h1, r1 = F.rmsnorm_fwd(x2, w_in, layer.eps)                                        # llama.py:296
-        qkv = torch.empty((B * S, 3 * D), device=x.device, dtype=BF16)
+        qkv = torch.empty((B * S, D + 2 * Dkv), device=x.device, dtype=BF16)
         F.linear_fwd(h1, P.bf16_of(a.q_proj.weight), out=qkv[:, :D])                       # :222-224
-        F.linear_fwd(h1, P.bf16_of(a.k_proj.weight), out=qkv[:, D:2 * D])
-        F.linear_fwd(h1, P.bf16_of(a.v_proj.weight), out=qkv[:, 2 * D:])
-        F.rope128_(qkv, H, S, 2, layer.rope_theta)                                         # :229-230
-        o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128))   # :241-246
+        F.linear_fwd(h1, P.bf16_of(a.k_proj.weight), out=qkv[:, D:D + Dkv])
+        F.linear_fwd(h1, P.bf16_of(a.v_proj.weight), out=qkv[:, D + Dkv:])
+        _rope(layer, qkv, S, False)                                                        # :229-230
+        o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128),
+                               **_kv_kw(layer))                                             # :241-246
         x1 = F.linear_fwd(o, P.bf16_of(a.o_proj.weight), residual=x2)                      # :254,304
         h2, r2 = F.rmsnorm_fwd(x1, w_post, layer.eps)                                      # :308
         g = F.linear_fwd(h2, P.bf16_of(m.gate_proj.weight))
@@ -65,13 +71,49 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         dh2 = F.linear_dgrad(du, P.bf16_of(m.up_proj.weight), residual=dh2)
         dx1 = F.rmsnorm_bwd(dh2, x1, r2, P.f32_of(layer.post_attention_layernorm.weight), add=dy2)
         do = F.linear_dgrad(dx1, P.bf16_of(a.o_proj.weight))
-        dqkv = F.lm_attn_bwd(do, qkv, o, lse, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128))
-        F.rope128_(dqkv, H, S, 2, layer.rope_theta, backward=True)
+        dqkv = F.lm_attn_bwd(do, qkv, o, lse, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128),
+                             **_kv_kw(layer))
+        _rope(layer, dqkv, S, True)
+        Dkv = layer.num_key_value_heads * 128
         dh1 = F.linear_dgrad(dqkv[:, :D], P.bf16_of(a.q_proj.weight))
-        dh1 = F.linear_dgrad(dqkv[:, D:2 * D], P.bf16_of(a.k_proj.weight), residual=dh1)
-        dh1 = F.linear_dgrad(dqkv[:, 2 * D:], P.bf16_of(a.v_proj.weight), residual=dh1)
+        dh1 = F.linear_dgrad(dqkv[:, D:D + Dkv], P.bf16_of(a.k_proj.weight), residual=dh1)
+        dh1 = F.linear_dgrad(dqkv[:, D + Dkv:], P.bf16_of(a.v_proj.weight), residual=dh1)
         dx = F.rmsnorm_bwd(dh1, x2, r1, P.f32_of(layer.input_layernorm.weight), add=dx1)
         return dx.view(dy.shape), None, None, None
+
+
+def _kv_kw(layer):
+    """Extra attention arguments: none for multi-head attention, so that path makes exactly the calls it always made."""
+    kv = layer.num_key_value_heads
+    return {} if kv == layer.num_heads else {"kv_heads": kv}
+
+
+def _rope(layer, buf, S, backward):
+    """Rotary embedding in place on the q and k blocks of the fused projection buffer (or of its gradient)."""
+    H, kv = layer.num_heads, layer.num_key_value_heads
+    if not layer.table_rope:                                   # multi-head attention, default RoPE: theta in the kernel
+        if backward:
+            F.rope128_(buf, H, S, 2, layer.rope_theta, backward=True)
+        else:
+            F.rope128_(buf, H, S, 2, layer.rope_theta)
+        return
+    inv, sc = layer.rope_inv_freq(buf.device), layer.rope_attention_scaling
+    if kv == H:
+        F.rope128_freqs_(buf, H, S, 2, inv, sc, backward=backward)
+    else:                                                      # q block (H heads), then k block (kv heads)
+        F.rope128_freqs_(buf[:, :H * 128], H, S, 1, inv, sc, backward=backward)
+        F.rope128_freqs_(buf[:, H * 128:(H + kv) * 128], kv, S, 1, inv, sc, backward=backward)
+
+
+def rope_table(hidden_size, num_attention_heads, rope_parameters, max_position_embeddings=None):
+    """(inv_freq fp32 [64] on the CPU, attention_scaling) of HF's LlamaRotaryEmbedding for these RoPE parameters."""
+    from transformers import LlamaConfig
+    from transformers.models.llama.modeling_llama import LlamaRotaryEmbedding
+    kw = {} if max_position_embeddings is None else {"max_position_embeddings": max_position_embeddings}
+    cfg = LlamaConfig(hidden_size=hidden_size, num_attention_heads=num_attention_heads, rope_parameters=dict(rope_parameters),
+                      **kw)
+    rot = LlamaRotaryEmbedding(cfg, device="cpu")
+    return rot.inv_freq.detach().float().clone(), float(rot.attention_scaling)
 
 
 class _RMSNormParams(nn.Module):
@@ -82,10 +124,10 @@ class _RMSNormParams(nn.Module):
 
 
 class _Attn(nn.Module):
-    def __init__(self, d):
+    def __init__(self, d, d_kv):
         super().__init__()
-        self.q_proj, self.k_proj = nn.Linear(d, d, bias=False), nn.Linear(d, d, bias=False)
-        self.v_proj, self.o_proj = nn.Linear(d, d, bias=False), nn.Linear(d, d, bias=False)
+        self.q_proj, self.k_proj = nn.Linear(d, d, bias=False), nn.Linear(d, d_kv, bias=False)
+        self.v_proj, self.o_proj = nn.Linear(d, d_kv, bias=False), nn.Linear(d, d, bias=False)
 
 
 class _MLP(nn.Module):
@@ -96,16 +138,44 @@ class _MLP(nn.Module):
 
 
 class FrozenLlamaDecoderLayer(nn.Module):
-    def __init__(self, hidden_size, num_attention_heads, intermediate_size, rms_norm_eps=1e-6, rope_theta=10000.0):
+    """num_key_value_heads: K/V heads (grouped-query attention; default: num_attention_heads).  rope_parameters: HF's
+    `config.rope_parameters` dict (rope_type default / linear / llama3 / yarn; default: {"rope_type": "default",
+    "rope_theta": rope_theta}); max_position_embeddings is passed to HF's RoPE initialisation (yarn may read it)."""
+
+    def __init__(self, hidden_size, num_attention_heads, intermediate_size, rms_norm_eps=1e-6, rope_theta=10000.0, *,
+                 num_key_value_heads=None, rope_parameters=None, max_position_embeddings=None):
         super().__init__()
         if hidden_size != num_attention_heads * 128:
             raise ValueError("FrozenLlamaDecoderLayer: head_dim must be 128 (LLaMA-7B: 4096 = 32 x 128)")
+        kv = num_attention_heads if num_key_value_heads is None else int(num_key_value_heads)
+        if kv <= 0 or num_attention_heads % kv != 0:
+            raise ValueError(f"FrozenLlamaDecoderLayer: num_key_value_heads = {kv} must divide {num_attention_heads} heads")
+        rp = dict(rope_parameters) if rope_parameters else {"rope_type": "default", "rope_theta": rope_theta}
+        rope_type = rp.get("rope_type", "default")
+        if rope_type not in _TABLE_ROPE_TYPES:
+            raise ValueError(f"FrozenLlamaDecoderLayer: rope_type {rope_type!r} is not covered (one of {_TABLE_ROPE_TYPES})")
+        rope_theta = rp.get("rope_theta", rope_theta)
         self.hidden_size, self.num_heads, self.eps, self.rope_theta = hidden_size, num_attention_heads, rms_norm_eps, rope_theta
-        self.self_attn = _Attn(hidden_size)
+        self.num_key_value_heads, self.rope_type = kv, rope_type
+        # multi-head attention with default RoPE keeps the theta-driven kernel; everything else uses HF's table
+        self.table_rope = not (kv == num_attention_heads and rope_type == "default")
+        self.rope_attention_scaling = 1.0
+        self._rope_freqs = {}                       # device -> fp32 [64] (plain attribute: module dtype casts leave it fp32)
+        if self.table_rope:
+            inv, self.rope_attention_scaling = rope_table(hidden_size, num_attention_heads, rp, max_position_embeddings)
+            self._rope_freqs[torch.device("cpu")] = inv
+        self.self_attn = _Attn(hidden_size, kv * 128)
         self.mlp = _MLP(hidden_size, intermediate_size)
         self.input_layernorm = _RMSNormParams(hidden_size, rms_norm_eps)
         self.post_attention_layernorm = _RMSNormParams(hidden_size, rms_norm_eps)
         self.requires_grad_(False)
+
+    def rope_inv_freq(self, device):
+        """The fp32 [64] inverse-frequency table on `device` (copied there once)."""
+        t = self._rope_freqs.get(device)
+        if t is None:
+            t = self._rope_freqs[device] = self._rope_freqs[torch.device("cpu")].to(device)
+        return t
 
     def forward(self, hidden_states, attention_mask=None, position_ids=None, past_key_value=None, past_key_values=None,
                 output_attentions=False, use_cache=False, **kwargs):
@@ -151,14 +221,19 @@ def _right_padding_check(module, args, kwargs):
     return None
 
 
+_TABLE_ROPE_TYPES = ("default", "linear", "llama3", "yarn")
+
+
 def swappable(cfg):
-    """True when the HF LlamaConfig describes layers this module covers (MHA, head_dim 128, default RoPE, no biases)."""
+    """True when the HF LlamaConfig describes layers this module covers: head_dim 128, multi-head or grouped-query
+    attention (num_key_value_heads divides num_attention_heads), default / linear / llama3 / yarn RoPE, no biases."""
     rp = getattr(cfg, "rope_parameters", None) or {}
     rope_type = rp.get("rope_type", "default") if isinstance(rp, dict) else "default"
     hd = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
+    kv = getattr(cfg, "num_key_value_heads", None) or cfg.num_attention_heads
     return (hd == 128 and cfg.hidden_size == cfg.num_attention_heads * 128
-            and getattr(cfg, "num_key_value_heads", cfg.num_attention_heads) == cfg.num_attention_heads
-            and rope_type == "default" and not getattr(cfg, "attention_bias", False) and not getattr(cfg, "mlp_bias", False)
+            and cfg.num_attention_heads % kv == 0
+            and rope_type in _TABLE_ROPE_TYPES and not getattr(cfg, "attention_bias", False) and not getattr(cfg, "mlp_bias", False)
             and getattr(cfg, "hidden_act", "silu") == "silu" and cfg.hidden_size % 64 == 0 and cfg.intermediate_size % 64 == 0)
 
 
@@ -170,8 +245,14 @@ def swap_llama_layers(llama_model, keep_hf_for_cache=True):
         raise ValueError("swap_llama_layers: this LlamaConfig is outside FrozenLlamaDecoderLayer's coverage (see swappable())")
     rp = getattr(cfg, "rope_parameters", None) or {}
     theta = rp.get("rope_theta", getattr(cfg, "rope_theta", 10000.0))
+    kv = getattr(cfg, "num_key_value_heads", None) or cfg.num_attention_heads
+    rope_kw = {}
+    if kv != cfg.num_attention_heads or rp.get("rope_type", "default") != "default":
+        rope_kw = dict(num_key_value_heads=kv, rope_parameters=rp,
+                       max_position_embeddings=getattr(cfg, "max_position_embeddings", None))
     for i, old in enumerate(model.layers):
-        new = FrozenLlamaDecoderLayer(cfg.hidden_size, cfg.num_attention_heads, cfg.intermediate_size, cfg.rms_norm_eps, theta)
+        new = FrozenLlamaDecoderLayer(cfg.hidden_size, cfg.num_attention_heads, cfg.intermediate_size, cfg.rms_norm_eps, theta,
+                                      **rope_kw)
         _share_parameters(new, old)
         new.requires_grad_(False)
         if keep_hf_for_cache:
