@@ -88,6 +88,13 @@ static int make_tmap_2d(CUtensorMap* map, const void* base, uint64_t rows, uint6
       return OTB_OK;
     }
   }
+  // The driver call needs a current context on this thread.  A thread that has made no runtime call yet (the autograd
+  // engine's device thread, when the first backward reaches this library before any torch kernel there) has none:
+  // make the device's primary context current through the runtime.
+  int dev = 0;
+  cudaError_t ce = cudaGetDevice(&dev);
+  if (ce == cudaSuccess) ce = cudaSetDevice(dev);
+  if (ce != cudaSuccess) return set_error(OTB_ERR_CUDA, "cudaSetDevice before cuTensorMapEncodeTiled: %s", cudaGetErrorString(ce));
   cuuint64_t dims[2] = {cols, rows};
   cuuint64_t strides[1] = {ld * esz};
   cuuint32_t box[2] = {box_cols, box_rows};

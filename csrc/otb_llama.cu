@@ -3,7 +3,8 @@
 //   reference: xformers_model/llama.py:74-89 (LlamaRMSNorm), :150-166 (rotate_half / apply_rotary_pos_emb),
 //              :169-185 (LlamaMLP: down(silu(gate(x)) * up(x))), :186-259 (attention), :262-320 (decoder layer)
 // HBM-bound element-wise passes around the wgmma GEMMs and the head-dim-128 causal attention kernel:
-//   rmsnorm fwd / bwd(dx)     y = x * rsqrt(mean(x^2) + eps) * w             (the LM is frozen: no weight gradient)
+//   rmsnorm fwd / bwd         y = x * rsqrt(mean(x^2) + eps) * w;  backward: dx, and optionally the weight gradient
+//                             (trainable decoder layers) through a deterministic two-stage column reduction
 //   rope (in place)           q, k columns of the fused projection buffer, rotate_half convention, head dim 128;
 //                             frequencies from theta, or from a table (linear / llama3 / yarn scaling) with a cos/sin factor
 //   swiglu fwd / bwd          h = silu(g) * u ;  dg = dh * u * silu'(g), du = dh * silu(g)
@@ -84,6 +85,106 @@ rmsnorm_bwd_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __re
       if (pa) o[i] += fa[i];
     }
     po[v] = pack8(o);
+  }
+}
+
+// Weight-gradient variant: dx as rmsnorm_bwd_kernel (the row code below is the same, so dx has the same bits) and
+// dw[j] = sum_r dy[r,j] * x[r,j] * rstd[r].  CTAs stride over groups of 8 rows, one warp per row; after the warps' dx of
+// a group, thread t adds the group's rows, in row order, into its columns of the CTA's partial sums (vectors t, t + 256,
+// ... of smem `colacc` [D]; the rows were just read, so they come from cache).  Each CTA writes its partials to
+// ws[blockIdx.x][D]; rmsnorm_wgrad_finalize_kernel sums them in chunk order: deterministic, no atomics.
+__global__ void __launch_bounds__(256)
+rmsnorm_bwd_wgrad_kernel(const bf16* __restrict__ dy, long long lddy, const bf16* __restrict__ x, long long ldx,
+                         const float* __restrict__ rstd_in, const float* __restrict__ w, const bf16* __restrict__ add,
+                         long long ldadd, bf16* __restrict__ dx, long long lddx, float* __restrict__ ws, int rows, int D) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float4 colacc4[];
+  float* colacc = reinterpret_cast<float*>(colacc4);
+  const int lane = threadIdx.x & 31;
+  const int nvec = D >> 3;
+  for (int v = threadIdx.x; v < nvec; v += 256) {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) colacc[v * 8 + i] = 0.f;
+  }
+  for (int grp = blockIdx.x; grp * 8 < rows; grp += gridDim.x) {
+    const int row = grp * 8 + (threadIdx.x >> 5);
+    if (row < rows) {
+      const uint4* px = reinterpret_cast<const uint4*>(x + static_cast<long long>(row) * ldx);
+      const uint4* pd = reinterpret_cast<const uint4*>(dy + static_cast<long long>(row) * lddy);
+      const float rstd = rstd_in[row];
+      float s = 0.f;
+      for (int v = lane; v < nvec; v += 32) {
+        float fx[8], fd[8];
+        unpack8(__ldg(px + v), fx);
+        unpack8(__ldg(pd + v), fd);
+        const float4 w0 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v), w1 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v + 1);
+        const float ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+        for (int i = 0; i < 8; ++i) s += fd[i] * ww[i] * fx[i] * rstd;
+      }
+      const float m = warp_sum(s) / D;
+      uint4* po = reinterpret_cast<uint4*>(dx + static_cast<long long>(row) * lddx);
+      const uint4* pa = add ? reinterpret_cast<const uint4*>(add + static_cast<long long>(row) * ldadd) : nullptr;
+      for (int v = lane; v < nvec; v += 32) {
+        float fx[8], fd[8], fa[8], o[8];
+        unpack8(__ldg(px + v), fx);
+        unpack8(__ldg(pd + v), fd);
+        if (pa) unpack8(__ldg(pa + v), fa);
+        const float4 w0 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v), w1 = __ldg(reinterpret_cast<const float4*>(w) + 2 * v + 1);
+        const float ww[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          o[i] = rstd * (fd[i] * ww[i] - fx[i] * rstd * m);
+          if (pa) o[i] += fa[i];
+        }
+        po[v] = pack8(o);
+      }
+    }
+    const int r0 = grp * 8, nr = min(8, rows - r0);
+    for (int v = threadIdx.x; v < nvec; v += 256) {
+      float acc[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] = colacc[v * 8 + i];
+      for (int r = 0; r < nr; ++r) {
+        const long long rr = r0 + r;
+        const float rs = __ldg(rstd_in + rr);
+        float fx[8], fd[8];
+        unpack8(__ldg(reinterpret_cast<const uint4*>(x + rr * ldx) + v), fx);
+        unpack8(__ldg(reinterpret_cast<const uint4*>(dy + rr * lddy) + v), fd);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] += fd[i] * (fx[i] * rs);
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) colacc[v * 8 + i] = acc[i];
+    }
+  }
+  float* wr = ws + static_cast<long long>(blockIdx.x) * D;
+  for (int v = threadIdx.x; v < nvec; v += 256) {
+    reinterpret_cast<float4*>(wr)[2 * v] = colacc4[2 * v];
+    reinterpret_cast<float4*>(wr)[2 * v + 1] = colacc4[2 * v + 1];
+  }
+}
+
+// dw[c] (+)= sum over the chunks of ws[chunk][c]: a CTA owns 32 columns, its 8 thread rows stride over the chunks, then a
+// fixed-order smem reduction (deterministic).
+__global__ void __launch_bounds__(256)
+rmsnorm_wgrad_finalize_kernel(const float* __restrict__ ws, float* __restrict__ dw, int D, int chunks, int accumulate) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float sw[8][32];
+  const int c = blockIdx.x * 32 + threadIdx.x;
+  float a = 0.f;
+  if (c < D) {
+    for (int k = threadIdx.y; k < chunks; k += 8) a += ws[static_cast<long long>(k) * D + c];
+  }
+  sw[threadIdx.y][threadIdx.x] = a;
+  __syncthreads();
+  if (threadIdx.y == 0 && c < D) {
+    float t = 0.f;
+#pragma unroll
+    for (int y = 0; y < 8; ++y) t += sw[y][threadIdx.x];
+    dw[c] = (accumulate ? dw[c] : 0.f) + t;
   }
 }
 
@@ -170,6 +271,8 @@ swiglu_bwd_kernel(const bf16* __restrict__ dh, long long lddh, const bf16* __res
   }
 }
 
+constexpr int kRmsWGradMaxD = 16384;     // the weight-gradient kernel's column partials live in smem: D fp32
+
 static inline int ew_grid(long long items) {
   long long g = (items + 255) / 256;
   const long long cap = static_cast<long long>(sm_count()) * 8;
@@ -199,6 +302,35 @@ extern "C" int otb_rmsnorm_bwd(const void* dy, int64_t lddy, const void* x, int6
                           (long long)lddy, static_cast<const bf16*>(x), (long long)ldx, rstd, weight,
                           static_cast<const bf16*>(add), (long long)ldadd, static_cast<bf16*>(dx), (long long)lddx, rows, D));
   count_launch();
+  OTB_CHECK_CUDA(cudaGetLastError());
+  return OTB_OK;
+}
+
+extern "C" int otb_rmsnorm_bwd_chunks(int rows, int D) {
+  if (rows <= 0 || D <= 0) return 1;
+  const int groups = (rows + 7) / 8, cap = 4 * sm_count();     // 4 CTAs of 8 warps per SM
+  return groups < cap ? groups : cap;
+}
+
+extern "C" int otb_rmsnorm_bwd_params(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* rstd,
+                                      const float* weight, const void* add, int64_t ldadd, void* dx, int64_t lddx,
+                                      float* dweight, int accumulate, float* ws, int rows, int D, void* stream) {
+  OTB_CHECK_ARG(dy && x && rstd && weight && dx && dweight && ws && rows > 0 && D > 0 && D % 8 == 0,
+                "otb_rmsnorm_bwd_params: bad argument");
+  OTB_CHECK_ARG(D <= kRmsWGradMaxD, "otb_rmsnorm_bwd_params: D = %d exceeds %d", D, kRmsWGradMaxD);
+  OTB_CHECK_ARG(lddy % 8 == 0 && ldx % 8 == 0 && lddx % 8 == 0 && (add == nullptr || ldadd % 8 == 0),
+                "otb_rmsnorm_bwd_params: bad ld");
+  OTB_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 15) == 0, "otb_rmsnorm_bwd_params: ws must be 16-byte aligned");
+  const int chunks = otb_rmsnorm_bwd_chunks(rows, D);
+  const int smem = D * static_cast<int>(sizeof(float));
+  OTB_CHECK_CUDA(ensure_dyn_smem(rmsnorm_bwd_wgrad_kernel, kRmsWGradMaxD * static_cast<int>(sizeof(float))));   // once
+  OTB_CHECK_CUDA(launch_k(rmsnorm_bwd_wgrad_kernel, dim3(chunks), dim3(256), smem, ST(stream), static_cast<const bf16*>(dy),
+                          (long long)lddy, static_cast<const bf16*>(x), (long long)ldx, rstd, weight,
+                          static_cast<const bf16*>(add), (long long)ldadd, static_cast<bf16*>(dx), (long long)lddx, ws, rows,
+                          D));
+  OTB_CHECK_CUDA(launch_k(rmsnorm_wgrad_finalize_kernel, dim3((D + 31) / 32), dim3(32, 8), 0, ST(stream),
+                          static_cast<const float*>(ws), dweight, D, chunks, accumulate));
+  count_launch(2);
   OTB_CHECK_CUDA(cudaGetLastError());
   return OTB_OK;
 }

@@ -285,7 +285,11 @@ int otb_fuyu_scatter(const void* word, const void* cont, const int64_t* idx, con
  * SURVEY.md 8f rank 1 — LLaMA decoder layer (the LM of OTTER-Video-LLaMA7B), element-wise passes around the GEMMs and
  * otb_lm_attn_*:  xformers_model/llama.py:74-89 (LlamaRMSNorm), :150-166 (rotate_half rotary embedding), :169-185 (SwiGLU MLP).
  *   otb_rmsnorm_fwd   y = x * rsqrt(mean(x^2) + eps) * weight ; rstd fp32 [rows] kept for backward (may be NULL)
- *   otb_rmsnorm_bwd   dx (+ add) — the LM is frozen, no weight gradient
+ *   otb_rmsnorm_bwd   dx (+ add)
+ *   otb_rmsnorm_bwd_params  the same dx, bit for bit, and the weight gradient dweight fp32 [D] (+)= sum over rows of
+ *                     dy * x * rstd (accumulate != 0 adds to it), from one read of dy and x: per-CTA column partials go to
+ *                     ws fp32 [chunks][D] (16-byte aligned, chunks = otb_rmsnorm_bwd_chunks(rows, D)) and a second pass
+ *                     sums them in a fixed order (deterministic, no atomics).  D <= 16384
  *   otb_rope128       in place on `nblk` column blocks of H heads x 128 (q and k of a [rows][3*H*128] buffer); position of
  *                     a row = row % S; backward != 0 applies the transposed rotation
  *   otb_rope128_freqs the same rotation with inv_freq fp32 [64] from a table (HF's linear / llama3 / yarn RoPE scaling)
@@ -296,6 +300,10 @@ int otb_rmsnorm_fwd(const void* x, int64_t ldx, const float* weight, void* y, in
                     float eps, void* stream);
 int otb_rmsnorm_bwd(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* rstd, const float* weight,
                     const void* add, int64_t ldadd, void* dx, int64_t lddx, int rows, int D, void* stream);
+int otb_rmsnorm_bwd_chunks(int rows, int D);
+int otb_rmsnorm_bwd_params(const void* dy, int64_t lddy, const void* x, int64_t ldx, const float* rstd, const float* weight,
+                           const void* add, int64_t ldadd, void* dx, int64_t lddx, float* dweight, int accumulate, float* ws,
+                           int rows, int D, void* stream);
 int otb_rope128(void* buf, int64_t ld, int64_t rows, int H, int S, int nblk, float rope_theta, int backward, void* stream);
 int otb_rope128_freqs(void* buf, int64_t ld, int64_t rows, int H, int S, int nblk, const float* inv_freq, float attn_scale,
                       int backward, void* stream);

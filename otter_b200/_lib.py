@@ -116,6 +116,8 @@ SIGNATURES = {
     "otb_media_from_clip": (_I, [_VP, _VP, _I, _VP, _I, _I, _I, _VP]),
     "otb_rmsnorm_fwd": (_I, [_VP, _I64, _VP, _VP, _I64, _VP, _I, _I, _F, _VP]),
     "otb_rmsnorm_bwd": (_I, [_VP, _I64, _VP, _I64, _VP, _VP, _VP, _I64, _VP, _I64, _I, _I, _VP]),
+    "otb_rmsnorm_bwd_chunks": (_I, [_I, _I]),
+    "otb_rmsnorm_bwd_params": (_I, [_VP, _I64, _VP, _I64, _VP, _VP, _VP, _I64, _VP, _I64, _VP, _I, _VP, _I, _I, _VP]),
     "otb_rope128": (_I, [_VP, _I64, _I64, _I, _I, _I, _F, _I, _VP]),
     "otb_rope128_freqs": (_I, [_VP, _I64, _I64, _I, _I, _I, _VP, _F, _I, _VP]),
     "otb_swiglu_fwd": (_I, [_VP, _I64, _VP, _I64, _VP, _I64, _I64, _I, _VP]),

@@ -520,14 +520,26 @@ def rmsnorm_fwd(x, weight, eps, want_rstd=True):
 
 
 @_on_device
-def rmsnorm_bwd(dy, x, rstd, weight, add=None):
+def rmsnorm_bwd(dy, x, rstd, weight, add=None, *, dweight=None, accumulate=False):
+    """-> dx.  With dweight (fp32 [D]) the weight gradient sum_rows dy * x * rstd is also written into it (added to it
+    with accumulate=True); dx is then the same, bit for bit."""
     dy2, x2 = _mat(dy, "dy"), _mat(x, "x")
     rows, D = x2.shape
     dx = torch.empty((rows, D), device=x.device, dtype=BF16)
     add2 = _mat(add, "add") if add is not None else None
-    check(_lib.load().otb_rmsnorm_bwd(_p(dy2), dy2.stride(0), _p(x2), x2.stride(0), _p(rstd), _p(weight), _p(add2),
-                                      add2.stride(0) if add2 is not None else 0, _p(dx), dx.stride(0), rows, D, _stream()),
-          "otb_rmsnorm_bwd")
+    lib = _lib.load()
+    if dweight is None:
+        check(lib.otb_rmsnorm_bwd(_p(dy2), dy2.stride(0), _p(x2), x2.stride(0), _p(rstd), _p(weight), _p(add2),
+                                  add2.stride(0) if add2 is not None else 0, _p(dx), dx.stride(0), rows, D, _stream()),
+              "otb_rmsnorm_bwd")
+        return dx
+    _req(dweight, torch.float32, "dweight")
+    if dweight.shape != (D,) or dweight.device != x.device:
+        raise _lib.OtbError(f"dweight must be fp32 [{D}] on {x.device}, got {tuple(dweight.shape)} on {dweight.device}")
+    ws = torch.empty(lib.otb_rmsnorm_bwd_chunks(rows, D) * D, device=x.device, dtype=torch.float32)
+    check(lib.otb_rmsnorm_bwd_params(_p(dy2), dy2.stride(0), _p(x2), x2.stride(0), _p(rstd), _p(weight), _p(add2),
+                                     add2.stride(0) if add2 is not None else 0, _p(dx), dx.stride(0), _p(dweight),
+                                     int(bool(accumulate)), _p(ws), rows, D, _stream()), "otb_rmsnorm_bwd_params")
     return dx
 
 

@@ -1,9 +1,12 @@
-"""Frozen LLaMA decoder layer on the otter_b200 kernels — SURVEY.md §8f rank 1 (the LM of OTTER-Video-LLaMA7B, config c3).
+"""LLaMA decoder layer on the otter_b200 kernels — SURVEY.md §8f rank 1 (the LM of OTTER-Video-LLaMA7B, config c3).
 
 Mirrors `LlamaDecoderLayer` (/root/reference/xformers_model/llama.py:262-320; the reference falls back to HF's identical
 `transformers.models.llama` classes when xformers is absent, modeling_otter.py:52-54): same sub-module and parameter names
 (`input_layernorm`, `self_attn.{q,k,v,o}_proj`, `post_attention_layernorm`, `mlp.{gate,up,down}_proj`), no biases.
-The layer is FROZEN in Otter (modeling_otter.py:897-905): backward produces the input gradient only.
+Otter freezes the LM by default (modeling_otter.py:897-905), and so do the constructor and swap_llama_layers: backward
+then produces the input gradient only.  Parameters set to `requires_grad` afterwards (`train_lang_encoder`,
+`train_full_model`, partial unfreezing) also receive their gradients: the seven wgrad GEMMs and the RMSNorm weight
+gradients (otb_rmsnorm_bwd_params), written through `params.GradSink`.
 
   RMSNorm -> q / k / v GEMMs into one [rows, (H + 2 kv) * 128] buffer -> rotary embedding in place (rotate_half,
      head dim 128) -> causal attention (otb_lm_attn_*, no key bias) -> o_proj GEMM (+residual)
@@ -32,7 +35,7 @@ BF16 = torch.bfloat16
 
 class _FrozenLlamaLayerFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, layer, B, S):
+    def forward(ctx, x, layer, B, S, *params):   # params: layer.parameters() when any of them trains, else empty
         a, m = layer.self_attn, layer.mlp
         D, H = layer.hidden_size, layer.num_heads
         Dkv = layer.num_key_value_heads * 128
@@ -52,25 +55,47 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         u = F.linear_fwd(h2, P.bf16_of(m.up_proj.weight))
         hh = F.swiglu_fwd(g, u)                                                            # :184
         y = F.linear_fwd(hh, P.bf16_of(m.down_proj.weight), residual=x1)                   # :309-310
-        ctx.layer, ctx.B, ctx.S = layer, B, S
-        ctx.save_for_backward(x2, r1, qkv, o, lse, x1, r2, g, u)
+        ctx.layer, ctx.B, ctx.S, ctx.params = layer, B, S, params
+        # the weight GEMMs' other operands (the RMSNorm outputs and the SwiGLU output, the bits the forward GEMMs read)
+        # are kept only when something trains
+        ctx.save_for_backward(x2, r1, qkv, o, lse, x1, r2, g, u, *((h1, h2, hh) if params else ()))
         return y.view(x.shape)
 
     @staticmethod
     def backward(ctx, dy):
         layer, B, S = ctx.layer, ctx.B, ctx.S
-        x2, r1, qkv, o, lse, x1, r2, g, u = ctx.saved_tensors
+        x2, r1, qkv, o, lse, x1, r2, g, u = ctx.saved_tensors[:9]
         a, m = layer.self_attn, layer.mlp
         D, H = layer.hidden_size, layer.num_heads
         dy2 = dy.reshape(B * S, D)
         if dy2.dtype != BF16 or not dy2.is_contiguous():
             dy2 = dy2.to(BF16).contiguous()
+        train = bool(ctx.params)
+        h1, h2, hh = ctx.saved_tensors[9:] if train else (None, None, None)
+        sink = P.GradSink() if train else None
+
+        def wgrad(lin, dout, inp):
+            if train:
+                P.linear_param_grads(sink, lin, dout, inp)
+
+        def rms_kw(norm):
+            """No extra arguments for a frozen norm weight: the frozen path's call, unchanged."""
+            if not (train and norm.weight.requires_grad):
+                return {}
+            gw, acc = sink.target_f32(norm.weight)
+            return {"dweight": gw, "accumulate": acc}
+
         dh = F.linear_dgrad(dy2, P.bf16_of(m.down_proj.weight))
+        wgrad(m.down_proj, dy2, hh)
         dg, du = F.swiglu_bwd(dh, g, u)
         dh2 = F.linear_dgrad(dg, P.bf16_of(m.gate_proj.weight))
         dh2 = F.linear_dgrad(du, P.bf16_of(m.up_proj.weight), residual=dh2)
-        dx1 = F.rmsnorm_bwd(dh2, x1, r2, P.f32_of(layer.post_attention_layernorm.weight), add=dy2)
+        wgrad(m.gate_proj, dg, h2)
+        wgrad(m.up_proj, du, h2)
+        dx1 = F.rmsnorm_bwd(dh2, x1, r2, P.f32_of(layer.post_attention_layernorm.weight), add=dy2,
+                            **rms_kw(layer.post_attention_layernorm))
         do = F.linear_dgrad(dx1, P.bf16_of(a.o_proj.weight))
+        wgrad(a.o_proj, dx1, o)
         dqkv = F.lm_attn_bwd(do, qkv, o, lse, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128),
                              **_kv_kw(layer))
         _rope(layer, dqkv, S, True)
@@ -78,7 +103,12 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         dh1 = F.linear_dgrad(dqkv[:, :D], P.bf16_of(a.q_proj.weight))
         dh1 = F.linear_dgrad(dqkv[:, D:D + Dkv], P.bf16_of(a.k_proj.weight), residual=dh1)
         dh1 = F.linear_dgrad(dqkv[:, D + Dkv:], P.bf16_of(a.v_proj.weight), residual=dh1)
-        dx = F.rmsnorm_bwd(dh1, x2, r1, P.f32_of(layer.input_layernorm.weight), add=dx1)
+        wgrad(a.q_proj, dqkv[:, :D], h1)                          # gradients after the inverse RoPE, as the dgrad
+        wgrad(a.k_proj, dqkv[:, D:D + Dkv], h1)
+        wgrad(a.v_proj, dqkv[:, D + Dkv:], h1)
+        dx = F.rmsnorm_bwd(dh1, x2, r1, P.f32_of(layer.input_layernorm.weight), add=dx1, **rms_kw(layer.input_layernorm))
+        if train:
+            return (dx.view(dy.shape), None, None, None) + tuple(sink.result(p) for p in ctx.params)
         return dx.view(dy.shape), None, None, None
 
 
@@ -138,7 +168,9 @@ class _MLP(nn.Module):
 
 
 class FrozenLlamaDecoderLayer(nn.Module):
-    """num_key_value_heads: K/V heads (grouped-query attention; default: num_attention_heads).  rope_parameters: HF's
+    """Drop-in for HF's `LlamaDecoderLayer`, constructed frozen; parameters set to `requires_grad` afterwards receive their
+    gradients too.  (The name is kept: checkpoints and isinstance checks use it.)
+    num_key_value_heads: K/V heads (grouped-query attention; default: num_attention_heads).  rope_parameters: HF's
     `config.rope_parameters` dict (rope_type default / linear / llama3 / yarn; default: {"rope_type": "default",
     "rope_theta": rope_theta}); max_position_embeddings is passed to HF's RoPE initialisation (yarn may read it)."""
 
@@ -195,7 +227,7 @@ class FrozenLlamaDecoderLayer(nn.Module):
             if position_ids.shape[-1] != S or not bool((position_ids.reshape(-1, S) == want).all()):
                 raise NotImplementedError("only the default position_ids (arange) are supported")
         xb = hidden_states if hidden_states.dtype == BF16 else hidden_states.to(BF16)
-        y = _FrozenLlamaLayerFn.apply(xb.contiguous(), self, B, S)
+        y = _FrozenLlamaLayerFn.apply(xb.contiguous(), self, B, S, *P.trainable_params(self))
         return y.to(hidden_states.dtype)          # HF 5.x decoder layers return the tensor (SURVEY.md §8a-7)
 
 

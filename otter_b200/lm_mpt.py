@@ -1,11 +1,14 @@
-"""Frozen MPT decoder layer on the otter_b200 kernels (SURVEY.md §8f rank 1).
+"""MPT decoder layer on the otter_b200 kernels (SURVEY.md §8f rank 1).
 
 Mirrors `MPTBlock` (/root/reference/src/otter_ai/models/mpt/blocks.py:23-88) — same sub-module and parameter names
 (`norm_1`, `attn.Wqkv`, `attn.out_proj`, `norm_2`, `ffn.up_proj`, `ffn.down_proj`), same `forward()` signature and
 return tuple — for the configuration OTTER-Image-MPT7B ships: multi-head attention, `attn_impl: torch` semantics
-(mpt/attention.py:22-84), ALiBi key bias, causal mask, erf-GELU MLP, dropouts 0.  The layer is FROZEN in Otter
-(modeling_otter.py:905 freezes the LM): backward produces the input gradient only — five dgrad GEMMs, the causal
-attention backward and two LayerNorm backwards; no wgrad, and the bf16 weight copies are cast once.
+(mpt/attention.py:22-84), ALiBi key bias, causal mask, erf-GELU MLP, dropouts 0.  Otter freezes the LM by default
+(modeling_otter.py:905), and so does the constructor: backward then produces the input gradient only — five dgrad GEMMs,
+the causal attention backward and two LayerNorm backwards.  `train_lang_encoder` / `train_full_model`
+(modeling_otter.py:851-908), or any partial unfreezing, sets `requires_grad` on some parameters: backward then also
+writes the gradients of exactly those parameters (wgrad GEMMs, bias column sums, LayerNorm gamma / beta) through
+`params.GradSink`, so they land in a `FlatGradBuffer` when one is installed.
 
 head_dim must be 128 (MPT-7B / LLaMA-7B); there is no CPU path.
 """
@@ -28,9 +31,19 @@ def alibi_slopes(n_heads, alibi_bias_max=8, device=None):
     return slopes.contiguous()
 
 
+def layernorm_param_grads(sink, weight, bias, dout, x, mean, rstd, gamma):
+    """gamma / beta gradients of an nn.LayerNorm, for those that require grad.  The input gradient is computed apart, by
+    the same call the frozen path makes, so it has the same bits either way."""
+    targets = [sink.target_f32(p) if p is not None and p.requires_grad else None for p in (weight, bias)]
+    for acc in sorted({t[1] for t in targets if t is not None}):   # one call, two if the sinks are in different states
+        gw, gb = (t[0] if t is not None and t[1] == acc else None for t in targets)
+        F.layernorm_bwd(dout, x, mean, rstd, gamma, want_dx=False, dgamma=torch.empty_like(gamma) if gw is None else gw,
+                        dbeta=gb, accumulate=acc)
+
+
 class _FrozenMPTBlockFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, blk, B, S):
+    def forward(ctx, x, blk, B, S, *params):     # params: blk.parameters() when any of them trains, else empty
         D, H = blk.d_model, blk.n_heads
         x2 = x.reshape(B * S, D)
         g1, b1 = P.f32_of(blk.norm_1.weight), blk._beta(blk.norm_1)
@@ -46,14 +59,15 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
         z = torch.empty((B * S, w_up.shape[0]), device=x.device, dtype=torch.bfloat16)
         h = F.linear_fwd(m, w_up, bias=blk._bias(blk.ffn.up_proj), act=1, aux_out=z)
         y = F.linear_fwd(h, w_down, bias=blk._bias(blk.ffn.down_proj), residual=x1)
-        ctx.blk, ctx.B, ctx.S = blk, B, S
-        ctx.save_for_backward(x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z)
+        ctx.blk, ctx.B, ctx.S, ctx.params = blk, B, S, params
+        # the weight GEMMs' other operands (LN outputs a, m and the GELU output h) are kept only when something trains
+        ctx.save_for_backward(x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z, *((a, m, h) if params else ()))
         return y.view(x.shape)
 
     @staticmethod
     def backward(ctx, dy):
         blk, B, S = ctx.blk, ctx.B, ctx.S
-        x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z = ctx.saved_tensors
+        x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z = ctx.saved_tensors[:10]
         D, H = blk.d_model, blk.n_heads
         dy2 = dy.reshape(B * S, D)
         if dy2.dtype != torch.bfloat16 or dy2.stride(-1) != 1:
@@ -61,14 +75,31 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
         g1, g2 = P.f32_of(blk.norm_1.weight), P.f32_of(blk.norm_2.weight)
         w_qkv, w_out = P.bf16_of(blk.attn.Wqkv.weight), P.bf16_of(blk.attn.out_proj.weight)
         w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
+        train = bool(ctx.params)
+        if train:
+            a, m, h = ctx.saved_tensors[10:]
+            sink = P.GradSink()
 
         dz = F.linear_dgrad(dy2, w_down, aux_in=z)                       # (dy W_down) * gelu'(z)
+        if train:
+            P.linear_param_grads(sink, blk.ffn.down_proj, dy2, h)
         dm = F.linear_dgrad(dz, w_up)
+        if train:
+            P.linear_param_grads(sink, blk.ffn.up_proj, dz, m)
         dx1, _, _ = F.layernorm_bwd(dm, x1, mean2, rstd2, g2, add=dy2, want_param_grads=False)   # + residual branch
+        if train:
+            layernorm_param_grads(sink, blk.norm_2.weight, blk.norm_2.bias, dm, x1, mean2, rstd2, g2)
         do = F.linear_dgrad(dx1, w_out)
+        if train:
+            P.linear_param_grads(sink, blk.attn.out_proj, dx1, o)
         dqkv = F.lm_attn_bwd(do, qkv, o, lse, B, S, H, slopes=blk.slopes, causal=True, scale=blk.softmax_scale)
         da = F.linear_dgrad(dqkv, w_qkv)
+        if train:
+            P.linear_param_grads(sink, blk.attn.Wqkv, dqkv, a)
         dx, _, _ = F.layernorm_bwd(da, x2, mean1, rstd1, g1, add=dx1, want_param_grads=False)
+        if train:
+            layernorm_param_grads(sink, blk.norm_1.weight, blk.norm_1.bias, da, x2, mean1, rstd1, g1)
+            return (dx.view(dy.shape), None, None, None) + tuple(sink.result(p) for p in ctx.params)
         return dx.view(dy.shape), None, None, None
 
 
@@ -87,7 +118,9 @@ class _MLP(nn.Module):
 
 
 class FrozenMPTBlock(nn.Module):
-    """Drop-in for a frozen `MPTBlock` (state-dict keys identical); trains nothing, propagates input gradients."""
+    """Drop-in for `MPTBlock` (state-dict keys identical).  Constructed frozen, as Otter uses it; parameters set to
+    `requires_grad` afterwards receive their gradients too.  (The name is kept: `_no_split_modules`, checkpoints and
+    isinstance checks use it.)"""
 
     def __init__(self, d_model, n_heads, expansion_ratio=4, no_bias=True, alibi=True, alibi_bias_max=8,
                  softmax_scale=None):
@@ -129,7 +162,7 @@ class FrozenMPTBlock(nn.Module):
             self.slopes = alibi_slopes(self.n_heads, self.alibi_bias_max, device=x.device)
         B, S, _ = x.shape
         xb = x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)
-        y = _FrozenMPTBlockFn.apply(xb.contiguous(), self, B, S)
+        y = _FrozenMPTBlockFn.apply(xb.contiguous(), self, B, S, *P.trainable_params(self))
         return (y, None, past_key_value)
 
 
@@ -142,7 +175,8 @@ class FrozenMPTBlock(nn.Module):
 # (`transformer.wte.weight`, `transformer.blocks.{i}.{norm_1,attn.Wqkv,attn.out_proj,norm_2,ffn.up_proj,
 # ffn.down_proj}.weight`, `transformer.norm_f.weight`), so reference checkpoints load unchanged.
 # Scope: the configuration OTTER-Image-MPT7B ships (ALiBi, multi-head attention, no biases, tied embeddings,
-# dropouts 0).  The decoder layers are frozen in Otter (modeling_otter.py:897-905): input gradients only.  The tied
+# dropouts 0).  The decoder layers and norm_f are frozen in Otter by default (modeling_otter.py:897-905): input gradients
+# only; unfrozen (train_lang_encoder / train_full_model) they also write their parameter gradients.  The tied
 # embedding IS trained there (:905): it receives the gather gradient (torch index op) and the un-embedding wgrad.
 # No KV cache: generate() re-runs the whole prefix each step (correct, O(n^2) — the decode path is not the hot path).
 # =================================================================================================
@@ -184,20 +218,27 @@ def _as_bf16(t):
 
 
 class _FrozenLayerNormFn(torch.autograd.Function):
-    """LayerNorm with frozen affine parameters: input gradient only (norm_f, modeling_mpt.py:292)."""
+    """LayerNorm (norm_f, modeling_mpt.py:292): input gradient, and the gamma / beta gradients of those that require grad
+    (`bias` is the bias Parameter or None; `beta` its fp32 value or zeros)."""
 
     @staticmethod
-    def forward(ctx, x2, w, beta):
+    def forward(ctx, x2, w, beta, bias=None):
         y, mean, rstd = F.layernorm_fwd(x2, P.f32_of(w), beta)
         ctx.save_for_backward(x2, mean, rstd)
-        ctx.w = w
+        ctx.w, ctx.bias = w, bias
         return y
 
     @staticmethod
     def backward(ctx, dy):
         x2, mean, rstd = ctx.saved_tensors
-        dx, _, _ = F.layernorm_bwd(_as_bf16(dy).contiguous(), x2, mean, rstd, P.f32_of(ctx.w), want_param_grads=False)
-        return dx, None, None
+        dy2 = _as_bf16(dy).contiguous()
+        dx, _, _ = F.layernorm_bwd(dy2, x2, mean, rstd, P.f32_of(ctx.w), want_param_grads=False)
+        w, bias = ctx.w, ctx.bias
+        if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[3]):
+            return dx, None, None, None
+        sink = P.GradSink()
+        layernorm_param_grads(sink, w, bias, dy2, x2, mean, rstd, P.f32_of(w))
+        return dx, sink.result(w), None, (sink.result(bias) if bias is not None else None)
 
 
 class _UnembedFn(torch.autograd.Function):
@@ -293,7 +334,8 @@ class MPTModel(nn.Module):
             if self._zeros is None or self._zeros.device != x.device:
                 self._zeros = torch.zeros(self.config.d_model, device=x.device, dtype=torch.float32)
             beta = self._zeros
-        x = _FrozenLayerNormFn.apply(x.reshape(B * S, -1).contiguous(), self.norm_f.weight, beta).view(B, S, -1)   # :292
+        bias = self.norm_f.bias if self.norm_f.bias is not None and self.norm_f.bias.requires_grad else None
+        x = _FrozenLayerNormFn.apply(x.reshape(B * S, -1).contiguous(), self.norm_f.weight, beta, bias).view(B, S, -1)   # :292
         if output_hidden_states:
             hs = hs + (x,)
         return BaseModelOutputWithPast(last_hidden_state=x, past_key_values=None, hidden_states=hs, attentions=None)

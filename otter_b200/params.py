@@ -169,9 +169,34 @@ class GradSink:
         self.returned[id(p)] = t
         return t, False
 
+    def target_f32(self, p):
+        """target() for a gradient a row-wise kernel writes (norm weights, biases): those need an fp32 sink."""
+        g, acc = self.target(p)
+        if g.dtype != torch.float32:
+            raise RuntimeError("only weights produced by one wgrad GEMM can take a bf16 gradient sink (FlatGradBuffer "
+                               "direct_params); norm weights and biases need an fp32 one")
+        return g, acc
+
     def result(self, p):
         """What backward() returns to autograd for this parameter."""
         t = self.returned.get(id(p))
         if t is None:
             return None
         return t if p.dtype == torch.float32 else t.to(p.dtype)
+
+
+def trainable_params(module):
+    """The module's parameters, as extra inputs of its autograd Function, when grad mode is on and any of them requires
+    grad (autograd then asks the Function for their gradients); () otherwise, which keeps the frozen path's inputs."""
+    ps = tuple(module.parameters())
+    return ps if torch.is_grad_enabled() and any(p.requires_grad for p in ps) else ()
+
+
+def linear_param_grads(sink, lin, dout, inp):
+    """Gradients of an nn.Linear's weight (wgrad GEMM) and bias (column sum), for those that require grad."""
+    if lin.weight.requires_grad:
+        g, acc = sink.target(lin.weight)
+        F.linear_wgrad(dout, inp, out=g, accumulate=acc)
+    if lin.bias is not None and lin.bias.requires_grad:
+        g, acc = sink.target_f32(lin.bias)
+        F.grouped_colsum(dout, 1, 1, out=g.view(1, -1), accumulate=acc)

@@ -150,11 +150,6 @@ def main():
 
     def out(rec):
         print(json.dumps(rec), flush=True)
-    # The autograd engine's device thread has no current CUDA context until something makes one current there; the
-    # library's tensor-map encoding (a driver call) then fails with CUDA_ERROR_INVALID_CONTEXT.  A cuBLAS backward
-    # sets the primary context on that thread, as any earlier backward through a torch matmul would in training.
-    w = torch.randn(8, 8, device="cuda", requires_grad=True)
-    (w @ w).sum().backward()
     parts = args.parts.split(",")
     if args.tree == HERE:
         out({"card": card()})
