@@ -313,6 +313,21 @@ int otb_swiglu_bwd(const void* dh, int64_t lddh, const void* g, int64_t ldg, con
                    int64_t lddg, void* du, int64_t lddu, int64_t rows, int I, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * LoRA adapter dropout (otter_b200/lora.py; peft's lora_dropout on the adapter input, tuners/lora/layer.py Linear.forward)
+ *   otb_lora_dropout_fwd      out = x * keep / (1 - p)
+ *   otb_lora_dropout_bwd_add  dx += g * keep / (1 - p)   (the forward's mask, regenerated: nothing is stored)
+ * x / g / out / dx: bf16 [rows][cols], row pitch ld (elements, multiple of 8, >= cols), cols % 8 == 0, 16-byte aligned;
+ * 0 <= p < 1.  Mask: element e = row * cols + col (the logical index: independent of ld and of the launch geometry) takes
+ * word e % 4 of Philox4x32-10(counter = {lo32(e / 4), hi32(e / 4), stream_id, 0}, key = {lo32(seed), hi32(seed)}) and
+ *   keep  iff  word >= (uint32_t)floor((double)p * 2^32)
+ * (p = 0 keeps every element).  1 / (1 - p) is evaluated in fp32; out = bf16(x * scale) and dx = bf16(fma(g, scale, dx))
+ * on kept elements, 0 and dx on dropped ones.  Stateless, no atomics; each adapter of a layer uses its own stream_id. */
+int otb_lora_dropout_fwd(const void* x, void* out, int64_t rows, int cols, int64_t ld, float p, uint64_t seed,
+                         uint32_t stream_id, void* stream);
+int otb_lora_dropout_bwd_add(const void* g, void* dx, int64_t rows, int cols, int64_t ld, float p, uint64_t seed,
+                             uint32_t stream_id, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * SURVEY.md 8f rank 3 — Persimmon / Fuyu decoder layer: split + qk-LayerNorm + partial rotary embedding.
  * Replaces fuyu/modeling_persimmon.py:277-303 (`_split_heads`, fused_layer_norm on q and k, fused_apply_rotary_emb on
  * the first rotary_dims of every head, non-interleaved).  fused: bf16 [rows][H][3][64] (query_key_value output);

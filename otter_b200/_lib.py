@@ -122,6 +122,8 @@ SIGNATURES = {
     "otb_rope128_freqs": (_I, [_VP, _I64, _I64, _I, _I, _I, _VP, _F, _I, _VP]),
     "otb_swiglu_fwd": (_I, [_VP, _I64, _VP, _I64, _VP, _I64, _I64, _I, _VP]),
     "otb_swiglu_bwd": (_I, [_VP, _I64, _VP, _I64, _VP, _I64, _VP, _I64, _VP, _I64, _I64, _I, _VP]),
+    "otb_lora_dropout_fwd": (_I, [_VP, _VP, _I64, _I, _I64, _F, C.c_uint64, C.c_uint32, _VP]),
+    "otb_lora_dropout_bwd_add": (_I, [_VP, _VP, _I64, _I, _I64, _F, C.c_uint64, C.c_uint32, _VP]),
     "otb_qkln_rope_ws_floats": (_I, []),
     "otb_qkln_rope_fwd": (_I, [_VP, _I64, _VP, _VP, _VP, _VP, _VP, _I64, _VP, _I64, _I, _I, _I, _F, _F, _VP]),
     "otb_qkln_rope_bwd": (_I, [_VP, _I64, _VP, _I64, _VP, _VP, _VP, _VP, _I64, _VP, _VP, _VP, _VP, _I, _VP, _I64, _I, _I,

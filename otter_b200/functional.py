@@ -586,6 +586,45 @@ def swiglu_bwd(dh, g, u):
 
 
 # ------------------------------------------------------------------------------------------------
+# LoRA adapter dropout (csrc/otb_lora.cu)
+# ------------------------------------------------------------------------------------------------
+def _dropout_args(a, b, p):
+    a, b = _mat(a, "x"), _mat(b, "out")
+    if a.shape != b.shape or a.stride(0) != b.stride(0):
+        raise _lib.OtbError(f"lora dropout: operands must share shape and row pitch, got {tuple(a.shape)} / "
+                            f"{a.stride(0)} and {tuple(b.shape)} / {b.stride(0)}")
+    if not 0.0 <= p < 1.0:
+        raise _lib.OtbError(f"lora dropout: p = {p} must be in [0, 1)")
+    return a, b
+
+
+@_on_device
+def lora_dropout(x, p, seed, stream_id, out=None):
+    """out = x * keep / (1 - p); the keep mask is a pure function of (seed, stream_id, row, col), see
+    otb_lora_dropout_fwd in include/otter_b200.h.  x and out share one row pitch; without `out`, a 2-D x gets an output
+    [rows, cols] with x's row pitch."""
+    if out is None:
+        if x.dim() == 2:
+            out = torch.empty((x.shape[0], max(x.stride(0), x.shape[1])), device=x.device, dtype=BF16)[:, :x.shape[1]]
+        else:
+            out = torch.empty(x.shape, device=x.device, dtype=BF16)
+    x2, o2 = _dropout_args(x, out, p)
+    check(_lib.load().otb_lora_dropout_fwd(_p(x2), _p(o2), x2.shape[0], x2.shape[1], x2.stride(0), float(p),
+                                           int(seed) & (2 ** 64 - 1), int(stream_id), _stream()), "otb_lora_dropout_fwd")
+    return out
+
+
+@_on_device
+def lora_dropout_bwd_add_(g, dx, p, seed, stream_id):
+    """In place: dx += g * keep / (1 - p), with the mask lora_dropout(., p, seed, stream_id) drew."""
+    g2, d2 = _dropout_args(g, dx, p)
+    check(_lib.load().otb_lora_dropout_bwd_add(_p(g2), _p(d2), g2.shape[0], g2.shape[1], g2.stride(0), float(p),
+                                               int(seed) & (2 ** 64 - 1), int(stream_id), _stream()),
+          "otb_lora_dropout_bwd_add")
+    return dx
+
+
+# ------------------------------------------------------------------------------------------------
 # Persimmon / Fuyu layer: split + qk-LayerNorm + partial RoPE (csrc/otb_persimmon.cu)
 # ------------------------------------------------------------------------------------------------
 @_on_device

@@ -28,6 +28,7 @@ import torch
 from torch import nn
 
 from . import functional as F
+from . import lora as L
 from . import params as P
 
 BF16 = torch.bfloat16
@@ -43,9 +44,18 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         w_in, w_post = P.f32_of(layer.input_layernorm.weight), P.f32_of(layer.post_attention_layernorm.weight)
         h1, r1 = F.rmsnorm_fwd(x2, w_in, layer.eps)                                        # llama.py:296
         qkv = torch.empty((B * S, D + 2 * Dkv), device=x.device, dtype=BF16)
-        F.linear_fwd(h1, P.bf16_of(a.q_proj.weight), out=qkv[:, :D])                       # :222-224
+        lq, lv = L.adapter(a.q_proj), L.adapter(a.v_proj)          # LoRA on q / v (otter_b200.lora), else None
+        seed = L.layer_seed(x.device, lq, lv)
+        xas = []                                                   # xa = dropout(h1) A^T of each adapter
+        if lq is None:
+            F.linear_fwd(h1, P.bf16_of(a.q_proj.weight), out=qkv[:, :D])                   # :222-224
+        else:
+            xas.append(L.kernel_fwd(h1, P.bf16_of(a.q_proj.weight), lq, qkv[:, :D], seed, 0))
         F.linear_fwd(h1, P.bf16_of(a.k_proj.weight), out=qkv[:, D:D + Dkv])
-        F.linear_fwd(h1, P.bf16_of(a.v_proj.weight), out=qkv[:, D + Dkv:])
+        if lv is None:
+            F.linear_fwd(h1, P.bf16_of(a.v_proj.weight), out=qkv[:, D + Dkv:])
+        else:
+            xas.append(L.kernel_fwd(h1, P.bf16_of(a.v_proj.weight), lv, qkv[:, D + Dkv:], seed, 1))
         _rope(layer, qkv, S, False)                                                        # :229-230
         o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=None, causal=True, scale=1.0 / math.sqrt(128),
                                **_kv_kw(layer))                                             # :241-246
@@ -56,9 +66,12 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         hh = F.swiglu_fwd(g, u)                                                            # :184
         y = F.linear_fwd(hh, P.bf16_of(m.down_proj.weight), residual=x1)                   # :309-310
         ctx.layer, ctx.B, ctx.S, ctx.params = layer, B, S, params
+        ctx.lora = (lq, lv, seed)
         # the weight GEMMs' other operands (the RMSNorm outputs and the SwiGLU output, the bits the forward GEMMs read)
-        # are kept only when something trains
-        ctx.save_for_backward(x2, r1, qkv, o, lse, x1, r2, g, u, *((h1, h2, hh) if params else ()))
+        # are kept only for the weights that train: a layer that trains only its LoRA adapters keeps h1 alone
+        keep = (h1 if L.needs_input(a.q_proj, a.k_proj, a.v_proj) else None,
+                h2 if L.needs_input(m.gate_proj, m.up_proj) else None, hh if L.needs_input(m.down_proj) else None)
+        ctx.save_for_backward(x2, r1, qkv, o, lse, x1, r2, g, u, *(keep if params else ()), *xas)
         return y.view(x.shape)
 
     @staticmethod
@@ -71,7 +84,8 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         if dy2.dtype != BF16 or not dy2.is_contiguous():
             dy2 = dy2.to(BF16).contiguous()
         train = bool(ctx.params)
-        h1, h2, hh = ctx.saved_tensors[9:] if train else (None, None, None)
+        h1, h2, hh = ctx.saved_tensors[9:12] if train else (None, None, None)
+        xas = list(ctx.saved_tensors[12 if train else 9:])
         sink = P.GradSink() if train else None
 
         def wgrad(lin, dout, inp):
@@ -103,6 +117,11 @@ class _FrozenLlamaLayerFn(torch.autograd.Function):
         dh1 = F.linear_dgrad(dqkv[:, :D], P.bf16_of(a.q_proj.weight))
         dh1 = F.linear_dgrad(dqkv[:, D:D + Dkv], P.bf16_of(a.k_proj.weight), residual=dh1)
         dh1 = F.linear_dgrad(dqkv[:, D + Dkv:], P.bf16_of(a.v_proj.weight), residual=dh1)
+        lq, lv, seed = ctx.lora
+        if lq is not None:                                        # LoRA: the adapters' share of dh1, A / B gradients
+            dh1 = L.kernel_bwd(sink, dqkv[:, :D], h1, xas.pop(0), lq, seed, 0, dh1)
+        if lv is not None:
+            dh1 = L.kernel_bwd(sink, dqkv[:, D + Dkv:], h1, xas.pop(0), lv, seed, 1, dh1)
         wgrad(a.q_proj, dqkv[:, :D], h1)                          # gradients after the inverse RoPE, as the dgrad
         wgrad(a.k_proj, dqkv[:, D:D + Dkv], h1)
         wgrad(a.v_proj, dqkv[:, D + Dkv:], h1)

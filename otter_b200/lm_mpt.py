@@ -18,6 +18,7 @@ import torch
 from torch import nn
 
 from . import functional as F
+from . import lora as L
 from . import params as P
 
 
@@ -52,7 +53,14 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
         w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
 
         a, mean1, rstd1 = F.layernorm_fwd(x2, g1, b1)
-        qkv = F.linear_fwd(a, w_qkv, bias=blk._bias(blk.attn.Wqkv))
+        lw = L.adapter(blk.attn.Wqkv)                               # LoRA on Wqkv (otter_b200.lora), else None
+        seed = L.layer_seed(x.device, lw)
+        if lw is None:
+            qkv = F.linear_fwd(a, w_qkv, bias=blk._bias(blk.attn.Wqkv))
+            xas = ()
+        else:
+            qkv = torch.empty((B * S, w_qkv.shape[0]), device=x.device, dtype=torch.bfloat16)
+            xas = (L.kernel_fwd(a, w_qkv, lw, qkv, seed, 0, bias=blk._bias(blk.attn.Wqkv)),)
         o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=blk.slopes, causal=True, scale=blk.softmax_scale)
         x1 = F.linear_fwd(o, w_out, bias=blk._bias(blk.attn.out_proj), residual=x2)
         m, mean2, rstd2 = F.layernorm_fwd(x1, g2, b2)
@@ -60,8 +68,12 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
         h = F.linear_fwd(m, w_up, bias=blk._bias(blk.ffn.up_proj), act=1, aux_out=z)
         y = F.linear_fwd(h, w_down, bias=blk._bias(blk.ffn.down_proj), residual=x1)
         ctx.blk, ctx.B, ctx.S, ctx.params = blk, B, S, params
-        # the weight GEMMs' other operands (LN outputs a, m and the GELU output h) are kept only when something trains
-        ctx.save_for_backward(x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z, *((a, m, h) if params else ()))
+        ctx.lora = (lw, seed)
+        # the weight GEMMs' other operands (LN outputs a, m and the GELU output h) are kept only for the weights that
+        # train: a block that trains only its LoRA adapter keeps a alone
+        keep = (a if L.needs_input(blk.attn.Wqkv) else None, m if L.needs_input(blk.ffn.up_proj) else None,
+                h if L.needs_input(blk.ffn.down_proj) else None)
+        ctx.save_for_backward(x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z, *(keep if params else ()), *xas)
         return y.view(x.shape)
 
     @staticmethod
@@ -76,8 +88,9 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
         w_qkv, w_out = P.bf16_of(blk.attn.Wqkv.weight), P.bf16_of(blk.attn.out_proj.weight)
         w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
         train = bool(ctx.params)
+        a, sink = None, None
         if train:
-            a, m, h = ctx.saved_tensors[10:]
+            a, m, h = ctx.saved_tensors[10:13]
             sink = P.GradSink()
 
         dz = F.linear_dgrad(dy2, w_down, aux_in=z)                       # (dy W_down) * gelu'(z)
@@ -94,6 +107,9 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
             P.linear_param_grads(sink, blk.attn.out_proj, dx1, o)
         dqkv = F.lm_attn_bwd(do, qkv, o, lse, B, S, H, slopes=blk.slopes, causal=True, scale=blk.softmax_scale)
         da = F.linear_dgrad(dqkv, w_qkv)
+        lw, seed = ctx.lora
+        if lw is not None:                                        # LoRA: the adapter's share of da, A / B gradients
+            da = L.kernel_bwd(sink, dqkv, a, ctx.saved_tensors[-1], lw, seed, 0, da)
         if train:
             P.linear_param_grads(sink, blk.attn.Wqkv, dqkv, a)
         dx, _, _ = F.layernorm_bwd(da, x2, mean1, rstd1, g1, add=dx1, want_param_grads=False)

@@ -154,7 +154,9 @@ class _OtterBase(OtterPreTrainedModel):
         self.post_init()
 
     def _wrap_lora(self, config):
-        from peft import LoraConfig, TaskType, get_peft_model     # same optional dependency as the reference
+        """The reference's peft LoRA (:808-829), built by otter_b200.lora: peft's module and state-dict layout, with the
+        adapters running on the otter_b200 decoder layers' kernels (peft's would be bypassed there)."""
+        from .lora import wrap_lora
         arch = self.lang_encoder.__class__.__name__
         short = {"LlamaForCausalLM": "llama", "OPTForCausalLM": "opt", "GPTJForCausalLM": "gptj",
                  "GPTNeoXForCausalLM": "gpt_neox", "MPTForCausalLM": "mpt", "MosaicGPT": "mpt"}[
@@ -162,9 +164,8 @@ class _OtterBase(OtterPreTrainedModel):
         targets = {"llama": ["q_proj", "v_proj"], "opt": ["q_proj", "v_proj"], "gptj": ["q_proj", "v_proj"],
                    "gpt_neox": ["query_key_value"], "mpt": ["Wqkv"]}[short]
         lc = config.lora_config
-        self.lang_encoder = get_peft_model(self.lang_encoder, LoraConfig(
-            r=lc["r"], lora_alpha=lc["lora_alpha"], lora_dropout=lc["lora_dropout"], task_type=TaskType.CAUSAL_LM,
-            target_modules=targets))
+        self.lang_encoder = wrap_lora(self.lang_encoder, r=lc["r"], lora_alpha=lc["lora_alpha"],
+                                      lora_dropout=lc["lora_dropout"], target_modules=targets)
         self.lang_encoder.__class__.__name__ = f"{arch}LoRA"
 
     # ---- accessors (:833-849) ----
