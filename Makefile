@@ -1,7 +1,7 @@
 # Same commands as __graft_entry__.build(): the sm_90a shared library (all kernels + C ABI) and the GEMM self-test.
 NVCC      ?= nvcc
 NVCCFLAGS ?= -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17
-SRCS      := csrc/otb_host.cu csrc/otb_gemm.cu csrc/otb_attn.cu csrc/otb_norm.cu csrc/otb_fp32.cu csrc/otb_loss.cu csrc/otb_attn_lm.cu csrc/otb_data.cu csrc/otb_persimmon.cu csrc/otb_xattn_fused.cu csrc/otb_llama.cu csrc/otb_fp32_bwd.cu csrc/otb_lora.cu
+SRCS      := csrc/otb_host.cu csrc/otb_gemm.cu csrc/otb_attn.cu csrc/otb_norm.cu csrc/otb_fp32.cu csrc/otb_loss.cu csrc/otb_attn_lm.cu csrc/otb_data.cu csrc/otb_persimmon.cu csrc/otb_xattn_fused.cu csrc/otb_llama.cu csrc/otb_fp32_bwd.cu csrc/otb_lora.cu csrc/otb_decode.cu
 LIB       := otter_b200/lib/libotter_b200.so
 
 all: $(LIB) build/selftest_gemm

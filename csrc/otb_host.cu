@@ -175,6 +175,7 @@ int otb_abi_sizeof(int which) {
     case 2: return (int)sizeof(otb_attn_grads);
     case 3: return (int)sizeof(otb_lm_attn_desc);
     case 4: return (int)sizeof(otb_lm_attn_grads);
+    case 5: return (int)sizeof(otb_lm_attn_decode_desc);
     default: return -1;
   }
 }

@@ -36,7 +36,8 @@ long long otb_launch_count(void);
  * under a mutex (SURVEY.md 8b "no global mutable state beyond a mutex-guarded descriptor cache"). */
 long long otb_tmap_cache_stat(int which);
 /* sizeof() of the ABI structs as the C compiler laid them out: 0 otb_gemm_epilogue, 1 otb_attn_desc,
- * 2 otb_attn_grads, 3 otb_lm_attn_desc, 4 otb_lm_attn_grads (binding self-check for FFI hosts). */
+ * 2 otb_attn_grads, 3 otb_lm_attn_desc, 4 otb_lm_attn_grads, 5 otb_lm_attn_decode_desc (binding self-check for FFI
+ * hosts). */
 int otb_abi_sizeof(int which);
 
 /* ---------------------------------------------------------------------------------------------
@@ -179,6 +180,50 @@ typedef struct otb_lm_attn_grads {
 
 int otb_lm_attn_fwd(const otb_lm_attn_desc* d, void* stream);
 int otb_lm_attn_bwd(const otb_lm_attn_desc* d, const otb_lm_attn_grads* g, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * KV-cache decode step of the MPT decoder layers (csrc/otb_decode.cu): one new token per sequence.
+ *
+ * Decode attention — mpt/attention.py:41-45 (the cached keys / values are concatenated in front of the new token's)
+ * and :22-84 at one query row.  q bf16 [B][H*128] (row pitch ld_q); the cache is addressed in place: key / value row j
+ * of sequence b, head h at k / v + b * kv_batch_stride + j * ld_kv + h*128 (elements), so one [B][capacity][2*H*128]
+ * buffer with K at column 0 and V at column H*128 serves both.  T = number of valid rows including the new token's;
+ * rows >= T are never read.  out bf16 [B][H*128] (row pitch ld_out).
+ *   score(j) = scale * q.k_j + alibi_slopes[h] * (j - (T-1))     (otb_lm_attn_fwd's definition at i = S-1 = T-1)
+ * fp32 softmax and accumulation on the CUDA cores (one query row leaves a 64-row tensor-core tile empty; the kernel is
+ * bound by the HBM read of the cache).  The keys are split over CTAs — the split count follows from T, B*H and the SM
+ * count — and the splits' (max, sum, output) are combined from ws in split order: no atomics, two runs give the same
+ * bits.  ws: fp32, 16-byte aligned, otb_lm_attn_decode_ws_floats(B, H, T) floats (132 per batch, head and split).
+ * Multi-head only (every query head has its own K / V head).
+ * ------------------------------------------------------------------------------------------- */
+typedef struct otb_lm_attn_decode_desc {
+  const void* q;
+  const void* k;
+  const void* v;
+  void* out;
+  float* ws;
+  const float* alibi_slopes; /* fp32 [H] or NULL */
+  int64_t ld_q, ld_out, kv_batch_stride, ld_kv;
+  int32_t B, H, T, head_dim;
+  float scale;
+  int32_t _pad;
+} otb_lm_attn_decode_desc;
+
+long long otb_lm_attn_decode_ws_floats(int B, int H, int T);
+int otb_lm_attn_decode(const otb_lm_attn_decode_desc* d, void* stream);
+
+/* Linear layer at 1 <= M <= 8 rows (the decode step's nn.Linear calls, mpt/attention.py:322,339 and mpt/blocks.py:19-20
+ * at batch x beams rows):
+ *   y[M][N] = act(x[M][K] . w[N][K]^T + bias[n]) * alpha + residual[m][n]
+ * bf16 x / w / residual / y, fp32 accumulation, fp32 bias [N] or NULL, act 0 none / 1 GELU(erf) (the formula of
+ * otb_gemm_bf16's act = 1), residual NULL or bf16 (row pitch ld_res).  Row pitches in elements: ldx, ldw >= K and
+ * multiples of 8, ld_out, ld_res >= N; x and w 16-byte aligned; N % 8 == 0, K % 8 == 0.  A row slice of a weight and a
+ * row of the KV cache as the output are addressed in place.  The weight is read once, in 16-byte vectors, by CUDA-core
+ * CTAs that each own a few output columns (a 128 x 128 GEMM tile would put N / 128 CTAs on 132 SMs): bound by the
+ * HBM read of w.  Deterministic (fixed-order reduction, no atomics). */
+int otb_linear_small_m(const void* x, int64_t ldx, const void* w, int64_t ldw, int M, int N, int K, float alpha,
+                       const float* bias, int act, const void* residual, int64_t ld_res, void* out, int64_t ld_out,
+                       void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Index / mask construction (integer, bit-exact):  modeling_otter.py:296-311

@@ -68,6 +68,16 @@ class LmAttnGrads(C.Structure):
     ]
 
 
+class LmAttnDecodeDesc(C.Structure):
+    _fields_ = [
+        ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p), ("out", C.c_void_p), ("ws", C.c_void_p),
+        ("alibi_slopes", C.c_void_p),
+        ("ld_q", C.c_int64), ("ld_out", C.c_int64), ("kv_batch_stride", C.c_int64), ("ld_kv", C.c_int64),
+        ("B", C.c_int32), ("H", C.c_int32), ("T", C.c_int32), ("head_dim", C.c_int32),
+        ("scale", C.c_float), ("_pad", C.c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/otter_b200.h declares
 _VP, _I, _I64, _F = C.c_void_p, C.c_int, C.c_int64, C.c_float
 SIGNATURES = {
@@ -83,6 +93,9 @@ SIGNATURES = {
     "otb_xattn_out_fused": (_I, [C.POINTER(AttnDesc), _VP, _I64, _VP, _VP, _I64, _VP, _I64, _VP, _I64, _I, _VP]),
     "otb_lm_attn_fwd": (_I, [C.POINTER(LmAttnDesc), _VP]),
     "otb_lm_attn_bwd": (_I, [C.POINTER(LmAttnDesc), C.POINTER(LmAttnGrads), _VP]),
+    "otb_lm_attn_decode_ws_floats": (C.c_longlong, [_I, _I, _I]),
+    "otb_lm_attn_decode": (_I, [C.POINTER(LmAttnDecodeDesc), _VP]),
+    "otb_linear_small_m": (_I, [_VP, _I64, _VP, _I64, _I, _I, _I, _F, _VP, _I, _VP, _I64, _VP, _I64, _VP]),
     "otb_text_time": (_I, [_VP, _I, _I, _I, _VP, _VP]),
     "otb_layernorm_fwd": (_I, [_VP, _I64, _VP, _VP, _VP, _I64, _VP, _VP, _I, _I, _F, _VP]),
     "otb_ln_chunks": (_I, [_I, _I]),
@@ -148,7 +161,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError here = header/library mismatch: fail loudly
         fn.restype = res
         fn.argtypes = args
-    for i, st in enumerate((GemmEpilogue, AttnDesc, AttnGrads, LmAttnDesc, LmAttnGrads)):
+    for i, st in enumerate((GemmEpilogue, AttnDesc, AttnGrads, LmAttnDesc, LmAttnGrads, LmAttnDecodeDesc)):
         if lib.otb_abi_sizeof(i) != C.sizeof(st):
             raise OtbError(f"ABI mismatch: {st.__name__} is {C.sizeof(st)} bytes in ctypes, "
                            f"{lib.otb_abi_sizeof(i)} in the library")

@@ -10,7 +10,7 @@ import functools
 import torch
 
 from . import _lib
-from ._lib import AttnDesc, AttnGrads, GemmEpilogue, LmAttnDesc, LmAttnGrads, check
+from ._lib import AttnDesc, AttnGrads, GemmEpilogue, LmAttnDecodeDesc, LmAttnDesc, LmAttnGrads, check
 
 BF16 = torch.bfloat16
 
@@ -211,6 +211,91 @@ def lm_attn_bwd(dout, qkv, out, lse, B, S, H, *, slopes=None, causal=True, scale
     g.dout_cols, g.dout_col0, g.dq_col0, g.dk_col0, g.dv_col0 = dout.shape[1], 0, 0, D, D + Dkv
     check(_lib.load().otb_lm_attn_bwd(C.byref(d), C.byref(g), _stream()), "otb_lm_attn_bwd")
     return dqkv
+
+
+# ------------------------------------------------------------------------------------------------
+# KV-cache decode step: one query row per (sequence, head) over the cache; linear layers at M <= 8 rows
+# ------------------------------------------------------------------------------------------------
+SMALL_M_MAX = 8          # otb_linear_small_m serves 1 .. 8 rows
+
+
+def _aligned16(t, name):
+    if t.data_ptr() % 16:
+        raise _lib.OtbError(f"{name} must be 16-byte aligned")
+    return t
+
+
+@_on_device
+def lm_attn_decode_splits(B, H, T):
+    """Number of key splits otb_lm_attn_decode uses for this shape on the current device."""
+    return int(_lib.load().otb_lm_attn_decode_ws_floats(B, H, T)) // (B * H * 132)
+
+
+@_on_device
+def lm_attn_decode(q, k, v, T, *, slopes=None, scale=None, out=None, ws=None):
+    """q bf16 [B, H*128]; k, v bf16 [B, capacity, H*128] views of the cache (any batch stride and row pitch that are
+    multiples of 8, e.g. the two column halves of one [B, capacity, 2*H*128] buffer); the first T rows are attended
+    (the new token's row is T-1), rows >= T are never read -> out bf16 [B, H*128]."""
+    q = _aligned16(_req(q, BF16, "q"), "q")
+    k, v = _aligned16(_req(k, BF16, "k"), "k"), _aligned16(_req(v, BF16, "v"), "v")
+    if q.dim() != 2 or q.shape[1] % 128 or k.dim() != 3 or k.shape != v.shape or k.stride() != v.stride():
+        raise _lib.OtbError(f"lm_attn_decode: q {tuple(q.shape)} / k {tuple(k.shape)} / v {tuple(v.shape)}: expected "
+                            "q [B, H*128] and k, v [B, capacity, H*128] with equal strides")
+    B, D = q.shape
+    if k.shape[0] != B or k.shape[2] != D or not 1 <= T <= k.shape[1]:
+        raise _lib.OtbError(f"lm_attn_decode: cache {tuple(k.shape)} does not hold T = {T} rows of q {tuple(q.shape)}")
+    if any(s % 8 for s in (q.stride(0), k.stride(0), k.stride(1))):
+        raise _lib.OtbError("lm_attn_decode: row pitches and the batch stride must be multiples of 8 elements")
+    H = D // 128
+    lib = _lib.load()
+    if slopes is not None:
+        _req(slopes, torch.float32, "alibi slopes")
+        assert slopes.shape == (H,), slopes.shape
+    if out is None:
+        out = torch.empty((B, D), device=q.device, dtype=BF16)
+    _req(out, BF16, "out")
+    assert out.shape == (B, D), out.shape
+    need = int(lib.otb_lm_attn_decode_ws_floats(B, H, T))
+    if ws is None:
+        ws = torch.empty(need, device=q.device, dtype=torch.float32)
+    _aligned16(_req(ws, torch.float32, "ws"), "ws")
+    if ws.numel() < need or not ws.is_contiguous():
+        raise _lib.OtbError(f"lm_attn_decode: workspace of {ws.numel()} floats, {need} needed")
+    d = LmAttnDecodeDesc()
+    d.q, d.k, d.v, d.out, d.ws, d.alibi_slopes = _p(q), _p(k), _p(v), _p(out), _p(ws), _p(slopes)
+    d.ld_q, d.ld_out, d.kv_batch_stride, d.ld_kv = q.stride(0), out.stride(0), k.stride(0), k.stride(1)
+    d.B, d.H, d.T, d.head_dim = B, H, T, 128
+    d.scale = (128 ** -0.5) if scale is None else scale
+    check(lib.otb_lm_attn_decode(C.byref(d), _stream()), "otb_lm_attn_decode")
+    return out
+
+
+@_on_device
+def linear_small_m(x, w, *, alpha=1.0, bias=None, act=0, residual=None, out=None):
+    """y[M,N] = act(x[M,K] @ w[N,K]^T + bias) * alpha + residual for 1 <= M <= 8 rows: the weight is streamed once by
+    CUDA-core CTAs that cover every SM (nn.Linear forward of a decode step).  x, w, residual and out may be row-pitched
+    views (a row slice of a fused weight, a row of the KV cache as `out`)."""
+    x, w = _aligned16(_req(x, BF16, "x"), "x"), _aligned16(_req(w, BF16, "w"), "w")
+    if x.dim() != 2 or w.dim() != 2 or w.shape[1] != x.shape[1]:
+        raise _lib.OtbError(f"linear_small_m: x {tuple(x.shape)} and w {tuple(w.shape)}: expected [M, K] and [N, K]")
+    M, K = x.shape
+    N = w.shape[0]
+    if not 1 <= M <= SMALL_M_MAX:
+        raise _lib.OtbError(f"linear_small_m: M = {M} must be in 1..{SMALL_M_MAX} (linear_fwd serves larger M)")
+    if bias is not None:
+        _req(bias, torch.float32, "bias")
+        assert bias.shape == (N,), bias.shape
+    if residual is not None:
+        _req(residual, BF16, "residual")
+        assert residual.shape == (M, N), residual.shape
+    if out is None:
+        out = torch.empty((M, N), device=x.device, dtype=BF16)
+    _req(out, BF16, "out")
+    assert out.shape == (M, N), out.shape
+    check(_lib.load().otb_linear_small_m(_p(x), x.stride(0), _p(w), w.stride(0), M, N, K, alpha, _p(bias), act,
+                                         _p(residual), residual.stride(0) if residual is not None else 0, _p(out),
+                                         out.stride(0), _stream()), "otb_linear_small_m")
+    return out
 
 
 # ------------------------------------------------------------------------------------------------

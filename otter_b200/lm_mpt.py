@@ -42,38 +42,44 @@ def layernorm_param_grads(sink, weight, bias, dout, x, mean, rstd, gamma):
                         dbeta=gb, accumulate=acc)
 
 
+def _block_forward(blk, x2, B, S):
+    """The block on B*S rows: the one forward body, of the autograd function and of the cached prefill.  Returns the output
+    and what the backward (and the KV cache: qkv) keeps."""
+    H = blk.n_heads
+    g1, b1 = P.f32_of(blk.norm_1.weight), blk._beta(blk.norm_1)
+    g2, b2 = P.f32_of(blk.norm_2.weight), blk._beta(blk.norm_2)
+    w_qkv, w_out = P.bf16_of(blk.attn.Wqkv.weight), P.bf16_of(blk.attn.out_proj.weight)
+    w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
+
+    a, mean1, rstd1 = F.layernorm_fwd(x2, g1, b1)
+    lw = L.adapter(blk.attn.Wqkv)                               # LoRA on Wqkv (otter_b200.lora), else None
+    seed = L.layer_seed(x2.device, lw)
+    if lw is None:
+        qkv = F.linear_fwd(a, w_qkv, bias=blk._bias(blk.attn.Wqkv))
+        xas = ()
+    else:
+        qkv = torch.empty((B * S, w_qkv.shape[0]), device=x2.device, dtype=torch.bfloat16)
+        xas = (L.kernel_fwd(a, w_qkv, lw, qkv, seed, 0, bias=blk._bias(blk.attn.Wqkv)),)
+    o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=blk.slopes, causal=True, scale=blk.softmax_scale)
+    x1 = F.linear_fwd(o, w_out, bias=blk._bias(blk.attn.out_proj), residual=x2)
+    m, mean2, rstd2 = F.layernorm_fwd(x1, g2, b2)
+    z = torch.empty((B * S, w_up.shape[0]), device=x2.device, dtype=torch.bfloat16)
+    h = F.linear_fwd(m, w_up, bias=blk._bias(blk.ffn.up_proj), act=1, aux_out=z)
+    y = F.linear_fwd(h, w_down, bias=blk._bias(blk.ffn.down_proj), residual=x1)
+    return y, (mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z), (a, m, h), xas, (lw, seed)
+
+
 class _FrozenMPTBlockFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, blk, B, S, *params):     # params: blk.parameters() when any of them trains, else empty
-        D, H = blk.d_model, blk.n_heads
-        x2 = x.reshape(B * S, D)
-        g1, b1 = P.f32_of(blk.norm_1.weight), blk._beta(blk.norm_1)
-        g2, b2 = P.f32_of(blk.norm_2.weight), blk._beta(blk.norm_2)
-        w_qkv, w_out = P.bf16_of(blk.attn.Wqkv.weight), P.bf16_of(blk.attn.out_proj.weight)
-        w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
-
-        a, mean1, rstd1 = F.layernorm_fwd(x2, g1, b1)
-        lw = L.adapter(blk.attn.Wqkv)                               # LoRA on Wqkv (otter_b200.lora), else None
-        seed = L.layer_seed(x.device, lw)
-        if lw is None:
-            qkv = F.linear_fwd(a, w_qkv, bias=blk._bias(blk.attn.Wqkv))
-            xas = ()
-        else:
-            qkv = torch.empty((B * S, w_qkv.shape[0]), device=x.device, dtype=torch.bfloat16)
-            xas = (L.kernel_fwd(a, w_qkv, lw, qkv, seed, 0, bias=blk._bias(blk.attn.Wqkv)),)
-        o, lse = F.lm_attn_fwd(qkv, B, S, H, slopes=blk.slopes, causal=True, scale=blk.softmax_scale)
-        x1 = F.linear_fwd(o, w_out, bias=blk._bias(blk.attn.out_proj), residual=x2)
-        m, mean2, rstd2 = F.layernorm_fwd(x1, g2, b2)
-        z = torch.empty((B * S, w_up.shape[0]), device=x.device, dtype=torch.bfloat16)
-        h = F.linear_fwd(m, w_up, bias=blk._bias(blk.ffn.up_proj), act=1, aux_out=z)
-        y = F.linear_fwd(h, w_down, bias=blk._bias(blk.ffn.down_proj), residual=x1)
+        x2 = x.reshape(B * S, blk.d_model)
+        y, saved, (a, m, h), xas, ctx.lora = _block_forward(blk, x2, B, S)
         ctx.blk, ctx.B, ctx.S, ctx.params = blk, B, S, params
-        ctx.lora = (lw, seed)
         # the weight GEMMs' other operands (LN outputs a, m and the GELU output h) are kept only for the weights that
         # train: a block that trains only its LoRA adapter keeps a alone
         keep = (a if L.needs_input(blk.attn.Wqkv) else None, m if L.needs_input(blk.ffn.up_proj) else None,
                 h if L.needs_input(blk.ffn.down_proj) else None)
-        ctx.save_for_backward(x2, mean1, rstd1, qkv, o, lse, x1, mean2, rstd2, z, *(keep if params else ()), *xas)
+        ctx.save_for_backward(x2, *saved, *(keep if params else ()), *xas)
         return y.view(x.shape)
 
     @staticmethod
@@ -117,6 +123,87 @@ class _FrozenMPTBlockFn(torch.autograd.Function):
             layernorm_param_grads(sink, blk.norm_1.weight, blk.norm_1.bias, da, x2, mean1, rstd1, g1)
             return (dx.view(dy.shape), None, None, None) + tuple(sink.result(p) for p in ctx.params)
         return dx.view(dy.shape), None, None, None
+
+
+# ---- KV cache and the cached decode step (inference only) ----
+def linear_rows(x, w, **epi):
+    """nn.Linear forward for the decode path: the weight-streaming kernel up to F.SMALL_M_MAX rows, the tensor-core GEMM
+    above (more beams than that make the 128-row tile worth its weight read)."""
+    return (F.linear_small_m if x.shape[0] <= F.SMALL_M_MAX else F.linear_fwd)(x, w, **epi)
+
+
+class MPTKVCache:
+    """Keys and values of every layer for `generate()`: per layer one bf16 [B][capacity][2*D] buffer, K of a token in
+    columns [0, D) and V in [D, 2*D) of its row — the layout of the K | V columns of the block's fused qkv row, so a
+    decode step's Wqkv[D:] projection writes its row in place.  All sequences of the batch have the same length
+    (`seq_len`); capacity grows geometrically by allocate-and-copy."""
+    is_compileable = False        # read by transformers' generate()
+
+    def __init__(self, n_layers):
+        self.layers = [None] * n_layers
+        self.seq_len = 0
+
+    def __len__(self):
+        return len(self.layers)
+
+    def get_seq_length(self, layer_idx=0):
+        return self.seq_len
+
+    @staticmethod
+    def grown_capacity(capacity, need):
+        """Capacity after a request for `need` rows: unchanged while it suffices, else at least doubled, in 64-row units."""
+        if need <= capacity:
+            return capacity
+        return (max(need, 2 * capacity) + 63) // 64 * 64
+
+    def reserve(self, need):
+        """Every layer can hold `need` rows; the first `seq_len` rows survive a growth."""
+        for i, buf in enumerate(self.layers):
+            cap = self.grown_capacity(buf.shape[1], need)
+            if cap != buf.shape[1]:
+                new = torch.empty((buf.shape[0], cap, buf.shape[2]), device=buf.device, dtype=buf.dtype)
+                new[:, :self.seq_len].copy_(buf[:, :self.seq_len])
+                self.layers[i] = new
+
+    def store_prefill(self, i, qkv, B, S):
+        """K | V columns of a prefill's qkv [B*S][3*D] -> layer i (allocated here, with room for the first new token)."""
+        D = qkv.shape[1] // 3
+        buf = torch.empty((B, self.grown_capacity(0, S + 1), 2 * D), device=qkv.device, dtype=qkv.dtype)
+        buf[:, :S].copy_(qkv.view(B, S, 3 * D)[:, :, D:])
+        self.layers[i] = buf
+
+    def reorder(self, beam_idx):
+        """Beam search: row b of the batch continues beam beam_idx[b] (modeling_mpt.py:495-504)."""
+        self.layers = [buf.index_select(0, beam_idx.to(buf.device)) for buf in self.layers]
+        return self
+
+
+def _block_decode(blk, x2, buf, T):
+    """One cached step of the block: x2 [B][D] is the new token's hidden state, buf the layer's cache with T - 1 valid
+    rows and room for row T - 1, which this call writes."""
+    D = blk.d_model
+    w_qkv, w_out = P.bf16_of(blk.attn.Wqkv.weight), P.bf16_of(blk.attn.out_proj.weight)
+    w_up, w_down = P.bf16_of(blk.ffn.up_proj.weight), P.bf16_of(blk.ffn.down_proj.weight)
+    b_qkv = blk._bias(blk.attn.Wqkv)
+    a, _, _ = F.layernorm_fwd(x2, P.f32_of(blk.norm_1.weight), blk._beta(blk.norm_1), want_stats=False)
+    row = buf[:, T - 1]                                         # [B][2*D], row pitch capacity * 2*D
+    lw = L.adapter(blk.attn.Wqkv)
+    if lw is None:
+        q = linear_rows(a, w_qkv[:D], bias=None if b_qkv is None else b_qkv[:D])
+        linear_rows(a, w_qkv[D:], bias=None if b_qkv is None else b_qkv[D:], out=row)
+    else:                                                       # + s (a A^T) B^T; adapter dropout is off in eval mode
+        A, Bw, s, _ = lw
+        Bw = P.bf16_of(Bw)
+        xa = linear_rows(a, P.bf16_of(A))
+        q = linear_rows(xa, Bw[:D], alpha=s,
+                        residual=linear_rows(a, w_qkv[:D], bias=None if b_qkv is None else b_qkv[:D]))
+        base = linear_rows(a, w_qkv[D:], bias=None if b_qkv is None else b_qkv[D:])
+        linear_rows(xa, Bw[D:], alpha=s, residual=base, out=row)
+    o = F.lm_attn_decode(q, buf[:, :, :D], buf[:, :, D:], T, slopes=blk.slopes, scale=blk.softmax_scale)
+    x1 = linear_rows(o, w_out, bias=blk._bias(blk.attn.out_proj), residual=x2)
+    m, _, _ = F.layernorm_fwd(x1, P.f32_of(blk.norm_2.weight), blk._beta(blk.norm_2), want_stats=False)
+    h = linear_rows(m, w_up, bias=blk._bias(blk.ffn.up_proj), act=1)
+    return linear_rows(h, w_down, bias=blk._bias(blk.ffn.down_proj), residual=x1)
 
 
 class _Attn(nn.Module):
@@ -166,19 +253,43 @@ class FrozenMPTBlock(nn.Module):
         return P.f32_of(lin.bias) if lin.bias is not None else None
 
     def forward(self, x, past_key_value=None, attn_bias=None, attention_mask=None, is_causal=True):
-        if past_key_value is not None or not is_causal:
-            raise NotImplementedError("FrozenMPTBlock: training path only (causal, no KV cache)")
+        """`past_key_value`: None, or (MPTKVCache, layer index) — the block then prefills that layer of an empty cache,
+        or runs one cached step on a single new token."""
+        if not is_causal:
+            raise NotImplementedError("FrozenMPTBlock: causal attention only")
+        cache = None
+        if past_key_value is not None:
+            if not (isinstance(past_key_value, tuple) and len(past_key_value) == 2
+                    and isinstance(past_key_value[0], MPTKVCache)):
+                raise NotImplementedError("FrozenMPTBlock: past_key_value must be (MPTKVCache, layer index)")
+            cache, layer = past_key_value
+            if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
+                raise NotImplementedError("FrozenMPTBlock: the KV cache is for inference (use torch.no_grad())")
+            if cache.seq_len > 0 and x.shape[1] != 1:
+                raise NotImplementedError("FrozenMPTBlock: a cached step takes one new token per sequence "
+                                          f"(got {x.shape[1]}: chunked prefill / assisted decoding are not implemented)")
         if attention_mask is not None:
             # Right padding needs no key mask under a causal mask (a real token never sees a later pad key, and the
             # ALiBi key bias is a per-row constant shift away from the relative form); anything else is refused.
             am = attention_mask.to(torch.bool)
+            if cache is not None and not bool(am.all()):
+                raise NotImplementedError("FrozenMPTBlock: the KV cache needs sequences of one length (no padding)")
             if not bool((am[:, 1:] <= am[:, :-1]).all()):
                 raise NotImplementedError("FrozenMPTBlock: only right-padded batches (no interior / left padding)")
         if self.alibi and (self.slopes is None or self.slopes.device != x.device):
             self.slopes = alibi_slopes(self.n_heads, self.alibi_bias_max, device=x.device)
         B, S, _ = x.shape
-        xb = x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)
-        y = _FrozenMPTBlockFn.apply(xb.contiguous(), self, B, S, *P.trainable_params(self))
+        xb = (x if x.dtype == torch.bfloat16 else x.to(torch.bfloat16)).contiguous()
+        if cache is None:
+            y = _FrozenMPTBlockFn.apply(xb, self, B, S, *P.trainable_params(self))
+        elif cache.seq_len == 0:                                  # prefill: today's forward, then K | V into the cache
+            with torch.no_grad():
+                y, saved, _, _, _ = _block_forward(self, xb.view(B * S, -1), B, S)
+                cache.store_prefill(layer, saved[2], B, S)
+                y = y.view(x.shape)
+        else:
+            with torch.no_grad():
+                y = _block_decode(self, xb.view(B, -1), cache.layers[layer], cache.seq_len + 1).view(x.shape)
         return (y, None, past_key_value)
 
 
@@ -194,7 +305,12 @@ class FrozenMPTBlock(nn.Module):
 # dropouts 0).  The decoder layers and norm_f are frozen in Otter by default (modeling_otter.py:897-905): input gradients
 # only; unfrozen (train_lang_encoder / train_full_model) they also write their parameter gradients.  The tied
 # embedding IS trained there (:905): it receives the gather gradient (torch index op) and the un-embedding wgrad.
-# No KV cache: generate() re-runs the whole prefix each step (correct, O(n^2) — the decode path is not the hot path).
+# KV cache: generate() decodes with an MPTKVCache by default, as transformers asks and the reference does
+# (prepare_inputs_for_generation, modeling_mpt.py:460-492): the prompt is prefilled by the forward below, then every step
+# runs ONE token through decode attention over the cache and the M <= 8 linear kernel.  Under Otter a cached step's
+# input_ids hold no <image> token, so the gated blocks' cross-attention rows are zero on those steps
+# (modeling_otter.py:326-330) and the tokens follow the reference's default.  generate(use_cache=False) and every direct
+# forward() (training, config.use_cache = False) re-run the whole prefix through the uncached path, bit for bit as before.
 # =================================================================================================
 from transformers import PretrainedConfig, PreTrainedModel  # noqa: E402
 from transformers.generation import GenerationMixin  # noqa: E402
@@ -317,6 +433,20 @@ class MPTModel(nn.Module):
             raise NotImplementedError("inputs_embeds is not implemented for MPT.")          # modeling_mpt.py:209-210
         if output_attentions:
             raise NotImplementedError("output_attentions is not implemented for the fused attention kernel")
+        use_cache = self.config.use_cache if use_cache is None else use_cache              # modeling_mpt.py:186
+        cache = past_key_values
+        if cache is not None and not isinstance(cache, MPTKVCache):
+            raise NotImplementedError("otter_b200 MPT: past_key_values must be an MPTKVCache (the one a forward with "
+                                      f"use_cache=True returned), got {type(cache).__name__}")
+        if cache is None and use_cache:
+            cache = MPTKVCache(self.config.n_layers)
+        if cache is not None and (self.training or (torch.is_grad_enabled() and any(
+                p.requires_grad for p in self.parameters()))):
+            raise NotImplementedError("otter_b200 MPT: the KV cache is for inference (eval mode under torch.no_grad())")
+        past = cache.seq_len if cache is not None else 0
+        if past and input_ids.size(1) != 1:
+            raise NotImplementedError("otter_b200 MPT: a cached step takes one new token per sequence (chunked prefill "
+                                      "and assisted decoding are not implemented)")
         if attention_mask is not None:
             # ONE host read per forward for both checks (the reference syncs here too, modeling_mpt.py:203): left
             # padding in training is the reference's error; interior padding is what the fused causal kernel cannot
@@ -324,25 +454,32 @@ class MPTModel(nn.Module):
             am = attention_mask.bool()
             left_pad = am[:, 0].sum() != am.shape[0]
             ragged = ~(am[:, 1:] <= am[:, :-1]).all()
-            left_pad, ragged = (bool(v) for v in torch.stack([left_pad, ragged]).tolist())
+            left_pad, ragged, padded = (bool(v) for v in torch.stack([left_pad, ragged, ~am.all()]).tolist())
             if left_pad and self.training:                                                 # modeling_mpt.py:203-204
                 raise NotImplementedError("MPT does not support training with left padding.")
+            if cache is not None and padded:
+                raise NotImplementedError("otter_b200 MPT: the KV cache needs sequences of one length (an "
+                                          "attention_mask of ones); pass use_cache=False for a padded batch")
             if left_pad or ragged:
                 raise NotImplementedError("otter_b200 MPT: only right-padded batches (no interior / left padding)")
             attention_mask = None
         S = input_ids.size(1)
-        assert S <= self.config.max_seq_len, \
-            f"Cannot forward input with seq_len={S}, this model only supports seq_len<={self.config.max_seq_len}"
+        assert S + past <= self.config.max_seq_len, \
+            f"Cannot forward input with seq_len={S + past}, this model only supports seq_len<={self.config.max_seq_len}"
         x = self.wte(input_ids)                                                            # :226 (ALiBi: no wpe)
         if self.embedding_fraction != 1:                                                   # :255-259
             x = x * self.embedding_fraction + x.detach() * (1 - self.embedding_fraction)
         x = _as_bf16(x)
+        if past:
+            cache.reserve(past + 1)
         hs = () if output_hidden_states else None
-        for block in self.blocks:                                                          # :270-283
+        for i, block in enumerate(self.blocks):                                            # :270-283
             if output_hidden_states:
                 hs = hs + (x,)
-            x, _, _ = block(x, past_key_value=None, attn_bias=None, attention_mask=attention_mask,
-                            is_causal=self.is_causal)
+            x, _, _ = block(x, past_key_value=None if cache is None else (cache, i), attn_bias=None,
+                            attention_mask=attention_mask, is_causal=self.is_causal)
+        if cache is not None:
+            cache.seq_len = past + S
         B = x.shape[0]
         if self.norm_f.bias is not None:
             beta = P.f32_of(self.norm_f.bias)
@@ -354,7 +491,7 @@ class MPTModel(nn.Module):
         x = _FrozenLayerNormFn.apply(x.reshape(B * S, -1).contiguous(), self.norm_f.weight, beta, bias).view(B, S, -1)   # :292
         if output_hidden_states:
             hs = hs + (x,)
-        return BaseModelOutputWithPast(last_hidden_state=x, past_key_values=None, hidden_states=hs, attentions=None)
+        return BaseModelOutputWithPast(last_hidden_state=x, past_key_values=cache, hidden_states=hs, attentions=None)
 
 
 class MPTPreTrainedModel(PreTrainedModel):
@@ -409,10 +546,10 @@ class MPTForCausalLM(MPTPreTrainedModel, GenerationMixin):
                 inputs_embeds=None, **unused):
         if inputs_embeds is not None:
             raise NotImplementedError("inputs_embeds has to be None (for hf/peft support).")   # modeling_mpt.py:398-399
-        out = self.transformer(input_ids=input_ids, past_key_values=None, attention_mask=attention_mask,
+        out = self.transformer(input_ids=input_ids, past_key_values=past_key_values, attention_mask=attention_mask,
                                prefix_mask=prefix_mask, sequence_id=sequence_id, return_dict=return_dict,
                                output_attentions=output_attentions, output_hidden_states=output_hidden_states,
-                               use_cache=False)
+                               use_cache=use_cache)
         h = out.last_hidden_state
         B, S, D = h.shape
         wte = self.transformer.wte.weight
@@ -420,19 +557,37 @@ class MPTForCausalLM(MPTPreTrainedModel, GenerationMixin):
         if V % 8:
             raise ValueError(f"vocab_size {V} must be a multiple of 8 for the tensor-core un-embedding "
                              "(resize_token_embeddings pads to a multiple of 8 for MPT's 50432-style vocabularies)")
-        logits = _UnembedFn.apply(h.reshape(B * S, D), wte).view(B, S, V)                     # :418-421
+        if out.past_key_values is not None:                # inference with a cache: B*S rows, nothing to differentiate
+            logits = linear_rows(h.reshape(B * S, D), P.bf16_of(wte)).view(B, S, V)
+        else:
+            logits = _UnembedFn.apply(h.reshape(B * S, D), wte).view(B, S, V)                 # :418-421
         if self.logit_scale is not None:
             logits = logits * self.logit_scale                                                  # :423-426
         loss = None
         if labels is not None:                                                                  # :428-436
             from .losses import shifted_cross_entropy
             loss = shifted_cross_entropy(logits, labels.to(logits.device))
-        return CausalLMOutputWithPast(loss=loss, logits=logits, past_key_values=None, hidden_states=out.hidden_states,
+        return CausalLMOutputWithPast(loss=loss, logits=logits, past_key_values=out.past_key_values,
+                                      hidden_states=out.hidden_states,
                                       attentions=None)
 
     def prepare_inputs_for_generation(self, input_ids, past_key_values=None, inputs_embeds=None, attention_mask=None,
                                       **kwargs):
-        """No KV cache: every decode step re-runs the whole prefix (modeling_mpt.py:456-483 minus the cache slice)."""
+        """modeling_mpt.py:460-492: with a cache only the last token is fed; `use_cache` defaults to True here, as in
+        the reference.  use_cache=False re-runs the whole prefix every step."""
         if inputs_embeds is not None:
             raise NotImplementedError("inputs_embeds is not implemented for MPT yet")
-        return {"input_ids": input_ids, "attention_mask": attention_mask, "past_key_values": None, "use_cache": False}
+        if past_key_values is not None:
+            input_ids = input_ids[:, -1].unsqueeze(-1)
+        return {"input_ids": input_ids, "attention_mask": attention_mask, "past_key_values": past_key_values,
+                "use_cache": kwargs.get("use_cache", True)}
+
+    @classmethod
+    def _supports_default_dynamic_cache(cls):
+        """The model builds its own cache (MPTKVCache): generate() must not hand it a transformers DynamicCache."""
+        return False
+
+    @staticmethod
+    def _reorder_cache(past_key_values, beam_idx):
+        """Beam search with the cache (modeling_mpt.py:495-504)."""
+        return past_key_values.reorder(beam_idx)
